@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- training images/sec of the BTS hot path on B200 (BASELINE.json metric), one JSON line.
+"""bench.py -- training images/sec of the BTS hot path on an H100 (BASELINE.json metric), one JSON line.
 
     python bench.py --gpus N --steps K --warmup W [--config K16|N4|R8|T1|LPG]    # our arm (torchrun launches N>1)
     python bench.py --impl reference --gpus N --steps K ...                      # reference arm: the reference on host cores
@@ -71,8 +71,8 @@ def peaks():
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d["bf16_tflops"],
                 "bf16_tflops_sustained": d.get("bf16_tflops_sustained", d["bf16_tflops"]),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+            "source": "fallback: NVIDIA H100 SXM data sheet (HBM3 3.35 TB/s, dense BF16 989 TFLOP/s at 700 W), not measured"}
 
 
 def synth_batch(cfg, B, seed, dev="cpu", pin=False):
@@ -113,7 +113,7 @@ def freeze_like_set_misc(model):
 
 
 class ClockSampler:
-    """nvidia-smi clocks + throttle reasons sampled DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks + throttle reasons sampled DURING the timed region."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
 
@@ -346,7 +346,7 @@ def _lpg_planes(torch, dev, Bn, h, w, r, max_depth):
 
 def _lpg_time(torch, dev, Bn, side, r, reps=20, flush=None):
     """average CUDA-event duration of bts_lpg_fwd / bts_lpg_bwd launched back to back through the C ABI.
-    flush: a buffer > L2 rewritten between launches (B=16 regime: working set < 126 MB L2, so each launch is timed alone)."""
+    flush: a buffer > L2 rewritten between launches (B=16 regime: working set < 50 MB L2, so each launch is timed alone)."""
     import ctypes
     from bts_b200 import _lib
     L = _lib.lib()
@@ -394,7 +394,7 @@ def _lpg_time(torch, dev, Bn, side, r, reps=20, flush=None):
 
 
 def lpg_roofline(torch, dev, pk):
-    """LPG fwd+bwd r=8/4/2 at 1024^2, batch 128: the output is 512 MB (>> 126 MB L2; consecutive launches cannot hit in
+    """LPG fwd+bwd r=8/4/2 at 1024^2, batch 128: the output is 512 MB (>> 50 MB L2; consecutive launches cannot hit in
     L2).  Algorithmic bytes: fwd 4*px*(1+4/r^2), bwd 4*px*(1+8/r^2)  (BASELINE.md section 3)."""
     out = {}
     for r in (8, 4, 2):
@@ -405,9 +405,6 @@ def lpg_roofline(torch, dev, pk):
     return {"bound": "hbm", "kernel": "lpg_fwd_vec<8> + lpg_bwd_vec<8> (fwd+bwd, r=8, 128x1024x1024, output 512 MB >> L2, "
                                       "20 back-to-back launches each, timed in isolation -> burst peak)",
             "achieved": a, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": a / pk["hbm_gbs"], "peak_source": pk["source"],
-            # dram__bytes_read.sum + dram__bytes_write.sum of one (fwd, bwd) launch pair, `ncu --set full` capture
-            # profiles/r01_lpg_r8_v2.ncu-rep of this same microbench: fwd 33.6 + 479.3 MB, bwd 570.4 + 32.3 MB
-            "traffic": 1115.6e6, "traffic_unit": "bytes per fwd+bwd launch pair (ncu, profiles/r01_lpg_r8_v2.ncu-rep)",
             "algorithmic_bytes": out["r8"]["algorithmic_bytes"], "sweep": out}
 
 
@@ -420,20 +417,20 @@ def run_lpg_config(args):
     from bts_b200 import _lib
     _lib.lib()
     pk = peaks()
-    flush = torch.zeros(64 * 1024 * 1024, device=dev)         # 256 MB > 126 MB L2
+    flush = torch.zeros(64 * 1024 * 1024, device=dev)         # 256 MB > 50 MB L2
     rows = []
     l0 = _lib.launches
     for r in (8, 4, 2):
         for side in (256, 384, 512, 768, 1024):
             Bh = max(16, (512 * 1024 * 1024 + 4 * side * side - 1) // (4 * side * side))
-            a = _lpg_time(torch, dev, Bh, side, r)
-            b = _lpg_time(torch, dev, 16, side, r, reps=10, flush=flush)
+            a = _lpg_time(torch, dev, Bh, side, r, reps=args.steps)
+            b = _lpg_time(torch, dev, 16, side, r, reps=args.steps, flush=flush)
             rows.append({"r": r, "side": side, "hbm": {k: a[k] for k in ("B", "fwd_ms", "bwd_ms", "fwd_gbs", "bwd_gbs", "fwd_bwd_gbs")},
                          "b16": {k: b[k] for k in ("B", "fwd_ms", "bwd_ms", "fwd_gbs", "bwd_gbs", "fwd_bwd_gbs")}})
             torch.cuda.empty_cache()
     vals = [x["hbm"]["fwd_bwd_gbs"] for x in rows]
     res = {"metric": "LPG fwd+bwd GB/s vs HBM peak", "value": statistics.median(vals), "unit": "GB/s", "n_gpus": 1,
-           "steps": 20, "warmup": 3, "ms_per_step": None, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
+           "steps": args.steps, "warmup": 3, "ms_per_step": None, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
            "dtype": "f32", "data": "synthetic",
            "config": {"workload": "LPG-u: plane-to-depth fwd+bwd, r=8/4/2, H=W 256..1024, 1 GPU; value = median over the 15 "
                                   "HBM-regime points", "l2": "hbm regime: outputs >= 512 MB; b16 regime: 256 MB flush write between launches"},
@@ -445,11 +442,11 @@ def run_lpg_config(args):
 
 
 # ------------------------------------------------------------------------------------------------ engine self-check
-# Round-2 fast paths (lean MMA issue loops, BatchNorm-backward sums in the dgrad epilogue, fused AdamW, CUDA-graph capture)
-# each have a switch.  Before timing, a SUBPROCESS checks each against an independent computation on the GPU at hand and the
+# The conv engine and the round-2 fast paths (BatchNorm-backward sums in the dgrad epilogue, fused AdamW, CUDA-graph capture)
+# are checked first; the fast paths each have a switch.  Before timing, a SUBPROCESS checks each against an independent computation on the GPU at hand and the
 # bench only enables what passed -- a kernel bug then costs speed and is reported in the JSON line ("selfcheck"), it does not
 # silently produce a wrong number or kill the run (a device-side trap in the child leaves this process's context intact).
-SELFCHECK_FEATURES = ["lean_issue", "bn_onepass", "epi_bnbwd", "fused_adamw"]
+SELFCHECK_FEATURES = ["conv_engine", "bn_onepass", "epi_bnbwd", "fused_adamw"]
 
 
 def selfcheck_child(enabled):
@@ -457,7 +454,7 @@ def selfcheck_child(enabled):
     import torch
     import torch.nn.functional as F
     from bts_b200 import _lib, conv, fused
-    L = _lib.lib()
+    _lib.lib()                                   # fail loudly if the CUDA library is missing
     dev = torch.device("cuda", 0)
     torch.backends.cudnn.allow_tf32 = False
     g = torch.Generator().manual_seed(0)
@@ -481,17 +478,10 @@ def selfcheck_child(enabled):
             worst = max(worst, relerr(y.detach(), yr.detach()), relerr(x.grad, xr.grad), relerr(w.grad, wr.grad))
         return worst < 2e-4, "worst rel-to-scale error %.2e vs torch fp32 conv (fwd/dgrad/wgrad, 4 layer shapes)" % worst
 
-    print("BEGIN lean_issue", flush=True)
-    L.bts_conv_set_issue_mode(1 if "lean_issue" in enabled else 0)
-    ok, det = engine_ok()
-    if "lean_issue" not in enabled:
-        print("CHECK lean_issue fail disabled after a crash; legacy loops: %s %s" % ("ok" if ok else "FAIL", det), flush=True)
-    elif not ok:
-        L.bts_conv_set_issue_mode(0)
-        ok2, det2 = engine_ok()
-        print("CHECK lean_issue fail %s; legacy loops: %s %s" % (det, "ok" if ok2 else "FAIL", det2), flush=True)
-    else:
-        print("CHECK lean_issue ok %s" % det, flush=True)
+    if "conv_engine" in enabled:
+        print("BEGIN conv_engine", flush=True)
+        ok, det = engine_ok()
+        print("CHECK conv_engine %s %s" % ("ok" if ok else "fail", det), flush=True)
 
     import torchvision
     blk = torchvision.models.densenet._DenseBlock(3, 64, 4, 32, 0.0).to(dev).train()
@@ -670,10 +660,12 @@ def _run_ours(args):
             ft = torch.tensor(flags, device=dev, dtype=torch.int32)
             dist.broadcast(ft, 0)
             flags = [int(v) for v in ft.tolist()]
-        lean_ok, onepass_ok, bnb_ok, adam_ok = [bool(v) for v in flags]
-        _lib.lib().bts_conv_set_issue_mode(1 if lean_ok else 0)
+        conv_ok, onepass_ok, bnb_ok, adam_ok = [bool(v) for v in flags]
+        if not conv_ok:                          # no alternative path: a wrong engine must not produce a throughput figure
+            raise SystemExit("bench.py: the conv engine failed its parity self-check (%s); no measurement reported"
+                             % (selfcheck["conv_engine"][1] if selfcheck else "reported by rank 0"))
         fused.BN_ONEPASS = fused.BN_ONEPASS and onepass_ok
-        fused.EPI_BNBWD = fused.EPI_BNBWD and bnb_ok      # off by default (measured slower, bts_b200/fused.py); opt-in via env
+        fused.EPI_BNBWD = fused.EPI_BNBWD and bnb_ok      # off by default (bts_b200/fused.py); opt-in via env
         if not adam_ok:
             args.optimizer = "torch"
     torch.backends.cudnn.benchmark = True        # bts_main.py:402
@@ -698,7 +690,7 @@ def _run_ours(args):
         model = torch.nn.parallel.DistributedDataParallel(model, device_ids=[local], find_unused_parameters=unused,
                                                           gradient_as_bucket_view=True)
     elif world > 1 and train:
-        # B200-native schedule (bts_b200/dist.py): ONE all-reduce of the flat gradient vector after backward and one flat
+        # native schedule (bts_b200/dist.py): ONE all-reduce of the flat gradient vector after backward and one flat
         # broadcast of rank 0's BatchNorm buffers before forward -- the same two collectives DDP issues (C1, C3 of SURVEY
         # 2.5), un-bucketed: the persistent 1-CTA-per-SM conv kernels leave NCCL no SM to overlap on anyway.
         from bts_b200 import dist as D
@@ -737,10 +729,14 @@ def _run_ours(args):
                 q.grad = None
             torch.cuda.synchronize()
 
+    last = {}                                    # what the last step computed (--dump-outputs)
+
     def step(i, x, f, g):
         if not train:
             with torch.no_grad():
-                return model(x, f)[4].sum()
+                depth = model(x, f)[4]
+                last["depth"] = depth
+                return depth.sum()
         if bcast is not None:
             bcast.broadcast(0)
         if graphed is not None:
@@ -756,6 +752,7 @@ def _run_ours(args):
         for grp in opt.param_groups:
             grp["lr"] = lr
         opt.step()
+        last["loss"] = loss
         return loss
 
     def timed(fn, K, Wm):
@@ -802,6 +799,8 @@ def _run_ours(args):
     K, Wm = args.steps, max(args.warmup, 3)
     ms, launches, clocks, per = timed(lambda i: step(i, img, focal, gt), K, Wm)
     rank_spans = getattr(timed, "rank_spans_ms", None)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, model, last, train)
 
     def e2e_step(i):
         if graphed is not None:                  # H2D straight into the graph's static input buffers
@@ -823,8 +822,8 @@ def _run_ours(args):
                    "collective": ("none" if world == 1 or not train else
                                   ("torch DDP (25 MB buckets, overlapped)" if args.reducer == "ddp" else
                                    "one NCCL all-reduce (AVG) of the flat gradient vector per step + one flat buffer broadcast")),
-                   "l2": "no explicit flush: per-step working set (saved activations, GBs) >> 126 MB L2",
-                   "precision": "3xTF32 split on tcgen05 (fp32-grade, parity mode)",
+                   "l2": "no explicit flush: per-step working set (saved activations, GBs) >> 50 MB L2",
+                   "precision": "3xTF32 split on wgmma (fp32-grade, parity mode)",
                    "cuda_graph": graph_note,
                    "optimizer": ("bts_b200.optim.FusedAdamW (one multi-tensor kernel + one re-pack launch)"
                                  if args.optimizer == "fused" else "torch.optim.AdamW") if train else "none"},
@@ -860,21 +859,11 @@ def _run_ours(args):
                         crit(o[4], gt, gt > cfg["thr"]).backward()
                     rl = conv_rooflines(torch, conv, eager_step, live)
                     if "conv" in rl:
-                        res["roofline"] = dict(rl["conv"], kernel="conv_tc_kernel (tcgen05 implicit GEMM: every conv forward and "
-                                                                  "dgrad of the step), all launches of one real training step",
-                                               # ncu --set full, profiles/r02_conv_db1_final.ncu-rep: dense 3x3 192->48 @88x176x16
-                                               # (the most frequent shape of the kernel), one launch: 191.1 MB read + 33.8 MB
-                                               # written vs 238.0 MB algorithmic (input 190.3 + output 47.6 + weights 0.08)
-                                               traffic=224.9e6, traffic_unit="bytes, ONE launch of the dense 3x3 192->48 layer (ncu "
-                                                                             "capture profiles/r02_conv_db1_final.ncu-rep; algorithmic "
-                                                                             "238 MB: no re-reads from DRAM; l1tex 82 %, tensor pipe 33 %)")
+                        res["roofline"] = dict(rl["conv"], kernel="conv_tc_kernel (wgmma implicit GEMM: every conv forward and "
+                                                                  "dgrad of the step), all launches of one real training step")
                     if "wgrad" in rl:
-                        res["roofline_wgrad"] = dict(rl["wgrad"], kernel="wgrad kernels (tcgen05, MN-major operands), all launches "
-                                                                         "of one real training step",
-                                                     # profiles/r02_wgrad2_db1_final.ncu-rep (dense 3x3 wgrad): 243.0 MB read + 3.8 MB written
-                                                     # vs 238.0 MB algorithmic (x 190.3 + dY 47.6); tensor pipe 72.6 %
-                                                     traffic=246.8e6, traffic_unit="bytes, ONE launch of the dense 3x3 192->48 wgrad (ncu, "
-                                                                                   "profiles/r02_wgrad2_db1_final.ncu-rep; algorithmic 238 MB)")
+                        res["roofline_wgrad"] = dict(rl["wgrad"], kernel="wgrad kernels (wgmma, operands transposed to K-major "
+                                                                         "by the producers), all launches of one real training step")
                 except Exception as e:
                     res["roofline"] = {"error": "%s: %s" % (type(e).__name__, e)}
             del model, opt
@@ -891,6 +880,32 @@ def _run_ours(args):
             if not args.no_cpu:
                 res["cpu_baseline"] = cpu_reference_steps(cfg, 3, 1)
     return res, rank, (dist if world > 1 else None)
+
+
+DUMP_SAMPLE = 4 << 20      # values per sampled array: 16 MB of float32 each, 32 MB in all
+
+
+def dump_outputs(path, model, last, train):
+    """Writes what the timed path computed in its last step as DIR/<name>.npy, so that two builds can be compared output
+    for output on the same seeded inputs: eval -> the final depth map; train -> the loss, and a fixed seeded sample of the
+    updated parameters and of their gradients (flattened in named_parameters order)."""
+    import numpy as np
+    import torch
+    os.makedirs(path, exist_ok=True)
+    torch.cuda.synchronize()
+    if not train:
+        np.save(os.path.join(path, "depth.npy"), last["depth"].detach().float().cpu().numpy())
+        return
+    np.save(os.path.join(path, "loss.npy"), np.array([float(last["loss"].detach())], dtype=np.float64))
+    m = model.module if hasattr(model, "module") else model
+    params = [q for _, q in m.named_parameters()]
+    flat = torch.cat([q.detach().reshape(-1) for q in params])
+    grads = torch.cat([(q.grad if q.grad is not None else torch.zeros_like(q)).detach().reshape(-1) for q in params])
+    rng = np.random.default_rng(0)
+    n = min(DUMP_SAMPLE, flat.numel())
+    idx = torch.from_numpy(np.sort(rng.choice(flat.numel(), n, replace=False))).to(flat.device)
+    np.save(os.path.join(path, "params_sample.npy"), flat[idx].float().cpu().numpy())
+    np.save(os.path.join(path, "grads_sample.npy"), grads[idx].float().cpu().numpy())
 
 
 def run_reference(args):
@@ -929,7 +944,14 @@ def main():
     ap.add_argument("--no-cpu", action="store_true", help="skip the CPU baseline leg")
     ap.add_argument("--no-gpu-baseline", action="store_true", help="skip the torch-eager/cuDNN reference leg")
     ap.add_argument("--no-roofline", action="store_true", help="skip every evidence leg (peaks, traced step, LPG, baselines)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last step computed as DIR/<name>.npy (float32 / float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be >= 1")
+    if args.dump_outputs and (args.impl == "reference" or args.config == "LPG"):
+        ap.error("--dump-outputs writes what the timed training / inference step computed; "
+                 "--impl reference and --config LPG have no such step")
     if args.selfcheck_child is not None:
         selfcheck_child(set(args.selfcheck_child.split(",")))
         return

@@ -2,7 +2,7 @@
 
 `bts_main.py` does `from bts import *` / `from bts import BtsModel` (bts_main.py:38,122-133) and
 `bts_test.py` imports `<model_name>.py` from the checkpoint directory (bts_test.py:68-74): putting this
-file (or a copy named <model_name>.py) on the import path swaps the whole model for the B200-native one.
+file (or a copy named <model_name>.py) on the import path swaps the whole model for the GPU-native one.
 The reference module also leaks `torch`, `nn`, `math`, `torch_nn_func` through `import *`; so do we.
 """
 import math  # noqa: F401

@@ -1,4 +1,4 @@
-"""bts_b200 -- B200-native (sm_100a) implementation of the BTS dense forward/backward hot path.
+"""bts_b200 -- GPU-native (H100, sm_90a) implementation of the BTS dense forward/backward hot path.
 
 Public surface = the reference's `bts` module surface (see bts_b200.model and the root-level bts.py);
 native boundary = the C ABI in include/bts_b200.h (libbts_b200.so, loaded by bts_b200._lib).

@@ -13,7 +13,7 @@ _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.path.join(_HERE, "libbts_b200.so")
 CSRC = os.path.join(_HERE, "csrc")
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
@@ -30,7 +30,7 @@ def needs_build():
 
 
 def build(force=False, verbose=False):
-    """nvcc cross-compiles every kernel for sm_100a into bts_b200/libbts_b200.so (works without a GPU)."""
+    """nvcc cross-compiles every kernel for sm_90a into bts_b200/libbts_b200.so (works without a GPU)."""
     if not force and not needs_build():
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
@@ -48,7 +48,7 @@ def build(force=False, verbose=False):
         out, _ = p.communicate()
         if p.returncode != 0:
             raise RuntimeError("nvcc failed on %s:\n%s" % (src, out.decode()))
-    cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH] + objs
+    cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH] + objs
     subprocess.check_call(cmd)
     return LIB_PATH
 
@@ -85,10 +85,10 @@ SIGNATURES = {
     "bts_bn_bwd_coef": [_p, _p, _ll, _i, _p, _p, _p, _p, _p],
     "bts_conv_set_tma": [_i],
     "bts_conv_get_tma": [],
-    "bts_conv_set_issue_mode": [_i],
     "bts_conv_set_producer_groups": [_i],
     "bts_conv_group_window": [_i, _i],
     "bts_conv_packed_floats_grouped": [_i, _i, _i, _i],
+    "bts_conv_group_n_tile": [_i],
     "bts_conv_pack_weights_grouped": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _i, _p, _p],
     "bts_conv_wgrad_grouped_plan": [_i, _i, _i, _i, _i, _i, _i, _p, _p],
     "bts_conv_wgrad_grouped": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _i, _p, _ll, _ll, _ll, _ll, _i, _p],

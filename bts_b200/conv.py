@@ -1,4 +1,4 @@
-"""Host side of the tcgen05 implicit-GEMM convolution engine (csrc/conv_tc.cu, C-ABI bts_conv_*).
+"""Host side of the wgmma implicit-GEMM convolution engine (csrc/conv_tc.cu, C-ABI bts_conv_*).
 
 Activations are NHWC in memory: torch tensors of logical shape (B,C,H,W) in `channels_last` format, so the same
 tensor is understood by the rest of torch (cat, BatchNorm, autograd) without transposes.  Weights keep the
@@ -108,7 +108,8 @@ def repack_cached():
             st = w.stride()
             if groups > 1:
                 kwin = group_window(Cout, Cin)
-                n_tile, n_tiles, cpg, ci_tot = kwin, Cout // kwin, Cin, Cout
+                n_tile = L.bts_conv_group_n_tile(kwin)
+                n_tiles, cpg, ci_tot = Cout // n_tile, Cin, Cout
             else:
                 rows = Cin if tf else Cout
                 n_tile = L.bts_conv_n_tile(rows)
@@ -138,8 +139,7 @@ CHUNK_MAJOR = _os.environ.get("BTS_B200_CHUNK_MAJOR", "0") == "1"
 def pack_flags(weight_shape, transpose_flip=False, groups=1):
     """packing / kernel flags of a layer.  bit 0 = chunk-major K order: for multi-tap kernels whose K channels are whole
     32-channel chunks, k-blocks run (chunk, tap) with the taps innermost, so the nine shifted reads of a pixel's channel chunk
-    are consecutive and hit in L1.  Measured on B200 (profiles/r02_*): L1 hit rate 77% and L2 throughput down to 11%, but the
-    kernel time did not move (the narrow layers are bound by shared-memory bandwidth, not L2), so it is off by default
+    are consecutive and hit in L1.  It is off by default: the narrow layers it targets are bound by operand staging, not L2
     (BTS_B200_CHUNK_MAJOR=1 enables it; tests/test_conv_order_gpu.py keeps it correct)."""
     Cout, Cin, KH, KW = weight_shape
     if not CHUNK_MAJOR or KH * KW == 1:
@@ -213,7 +213,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
     whose input was HxW -- the source is read as its zero-stuffed x2 expansion (use with transpose_flip, stride 1)."""
     _need_cuda(x, weight)
     if x.dtype != torch.float32:
-        raise TypeError("conv2d_tc computes in fp32 (3xTF32 on tcgen05); got %s" % x.dtype)
+        raise TypeError("conv2d_tc computes in fp32 (3xTF32 on wgmma); got %s" % x.dtype)
     x, xs = _nhwc_view(x)
     B, Cin, Hs, Ws = x.shape
     Co, Ci, KH, KW = weight.shape
@@ -344,7 +344,7 @@ def wgrad_grouped_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, d
 
 def wgrad_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=1, pre_scale=None, pre_shift=None,
              pre_relu=False, upsample2=False, precision=0):
-    """dW (shaped/strided like the weight parameter) on the tcgen05 engine."""
+    """dW (shaped/strided like the weight parameter) on the wgmma engine."""
     _need_cuda(x, gy)
     x, xs = _nhwc_view(x)
     gy, gs = _nhwc_view(gy)
@@ -387,9 +387,9 @@ def wgrad_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=
 
 
 class _ConvTC(torch.autograd.Function):
-    """Plain convolution (no fused pre/post ops) with autograd, all three GEMMs on the tcgen05 engine: forward,
+    """Plain convolution (no fused pre/post ops) with autograd, all three GEMMs on the wgmma engine: forward,
     dgrad (the same kernel over the transposed, tap-flipped packed operator; a stride-2 layer's dgrad reads dY as its
-    zero-stuffed expansion) and wgrad (MN-major operands).  groups > 1: block-diagonal operator (ResNeXt)."""
+    zero-stuffed expansion) and wgrad (operands transposed to K-major on their way into shared memory).  groups > 1: block-diagonal operator (ResNeXt)."""
 
     @staticmethod
     def forward(ctx, x, weight, stride, padding, dilation, groups):

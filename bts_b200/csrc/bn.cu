@@ -1,5 +1,5 @@
 // Train-mode BatchNorm pieces for the fused BN -> ReLU -> conv chains (DenseNet dense layers `norm1/relu1/conv1/norm2/
-// relu2/conv2`, torchvision densenet.py; decoder BNs pytorch/bts.py:154-182), sm_100a, HBM-bound.
+// relu2/conv2`, torchvision densenet.py; decoder BNs pytorch/bts.py:154-182), sm_90a, HBM-bound.
 //
 // The normalisation itself never runs as a kernel: it is folded into the consumer conv's A-operand prologue
 // (conv_tc.cu, PRE = affine + ReLU) as y = x*scale + shift with scale = gamma*invstd, shift = beta - mean*scale.

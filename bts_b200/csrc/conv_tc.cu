@@ -1,4 +1,4 @@
-// Implicit-GEMM convolution on the 5th-gen tensor cores (tcgen05 + TMEM), sm_100a, parity-grade 3xTF32.
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma, register accumulators), sm_90a, parity-grade 3xTF32.
 //
 // Replaces the cuDNN convolution (+ separate BN-apply / ReLU / ELU / nearest-upsample ATen kernels) behind every
 // 1x1 / 3x3 / dilated conv of the BTS decoder and the torchvision encoder (reference pytorch/bts.py:51-80,153-194).
@@ -10,32 +10,30 @@
 //              (upconv, bts.py:77) which is folded into the address map -- the 4x tensor is never materialised.
 //       act  = none | ELU | sigmoid, fused in the epilogue.
 //
-// GEMM view: M = B*Hout*Wout pixels (128 per CTA tile = the 128 TMEM lanes), N = Cout (<=256 per tile),
-// K = the dense sequence of 16-byte channel quads, tap-major, in blocks of 32 fp32 (one 128-byte swizzled row per pixel).
+// GEMM view: M = B*Hout*Wout pixels (128 per CTA tile: two warpgroups of 64 rows), N = Cout (<= 64 per tile: the
+// k-block accumulator and the tile sum of a 64 x 64 tile are 64 registers per thread), K = the dense sequence of 16-byte channel quads,
+// tap-major, in blocks of 32 fp32 (one 128-byte swizzled row per pixel).
 // Precision: fp32 operands are split x = hi + lo with hi = rna_tf32(x), lo = rna_tf32(x - hi) and the tile
-// accumulates  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with kind::tf32 MMAs into fp32 TMEM accumulators (error
-// ~2^-21 per product: fp32-grade, SURVEY Appendix F).  For N <= 128, A_hi*[B_hi;B_lo] is
-// ONE instruction of width 2N (the epilogue adds the two column blocks) and A_lo*B_hi the second -- a tcgen05.mma of
-// this shape costs ~120 cycles whatever N is, so the MMA count, not the FLOP count, sets the speed (see the MMA issuer).
+// accumulates  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with tf32 wgmma into fp32 register accumulators (error
+// ~2^-21 per product: fp32-grade, SURVEY Appendix F); every k-block's tensor-core sum is added into the tile sum with
+// round-to-nearest fp32 adds.
 // Single-pass TF32 is available as an explicitly labelled fast mode (precision=1) and is NOT used for parity.
 //
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... with the smem stage
-// ring, the two TMEM accumulators and all warp roles running continuously across tile boundaries (the MMA of tile
-// t+1 overlaps the epilogue of tile t; no per-tile launch / TMEM-alloc / pipeline-fill cost -- measured ~10 k cycles
-// per tile in the one-tile-per-CTA version, which dominated every small-K layer).
-// Warp roles (448 threads, 1 CTA/SM):
-//   warp 0      : weight loader -- one elected thread streams pre-packed, pre-split, pre-swizzled weight tiles
-//                 with 1-D bulk async copies (cp.async.bulk -> UBLKCP) completing on an mbarrier;
-//   warp 1      : TMEM allocator + MMA issuer -- one elected thread issues tcgen05.mma, commits to mbarriers;
-//   warps 2..9  : two producer groups (alternating k-blocks): coalesced 128-bit global loads of the activation
+// ring and all warp roles running continuously across tile boundaries (the loader and producers fill the stages of tile
+// t+1 while the consumers run the epilogue of tile t; no per-tile launch or pipeline-fill cost).
+// Warp roles (288 + 128 G threads, 1 CTA/SM):
+//   warps 0..7  : two consumer warpgroups -- wgmma on the staged operands, then the epilogue from the accumulator
+//                 registers: activation, NHWC stores, optional BatchNorm batch statistics of the output;
+//   warp 8      : weight loader -- one thread streams pre-packed, pre-split, pre-swizzled weight tiles with 1-D bulk
+//                 async copies (cp.async.bulk) completing on an mbarrier (and, in TMA mode, the im2col activation tile);
+//   warps 9..   : G producer groups (alternating k-blocks): coalesced 128-bit global loads of the activation
 //                 tile (8 lanes cover one pixel's 128 B), pre-op + hi/lo split in registers, swizzled 128-bit
-//                 shared stores of both halves, fence.proxy.async, mbarrier arrive;
-//   warps 10..13: epilogue: wait for the tile's accumulator, tcgen05.ld of the 128 rows, hi/lo block add, activation,
-//                 vectorised NHWC stores, optional BatchNorm batch statistics of the output, then hand the TMEM
-//                 accumulator back to the MMA warp.
+//                 shared stores of both halves, fence.proxy.async, mbarrier arrive.
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 
 #include <cuda.h>
 
@@ -45,14 +43,13 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 32;                 // fp32 elements per k-block = one 128-byte row
-constexpr int MAX_N = 256;                  // one tcgen05.mma covers up to 256 output channels
+constexpr int MAX_N = 64;                   // output channels per tile (two register accumulators per consumer thread)
 constexpr int A_TILE_BYTES = BLOCK_M * 128; // 16 KB (hi or lo)
-constexpr int NUM_THREADS = 448;
+constexpr int CONSUMER_THREADS = 256;       // two warpgroups
+constexpr int LOADER_WARP = CONSUMER_THREADS / 32;
 constexpr int PRODUCER_THREADS = 128;       // per group
+constexpr int FOUR_GROUPS_MAX_N = 48;       // widest tile run with four producer groups
 constexpr int MAX_CIN_SMEM = 4096;          // pre-op scale/shift staged in smem (32 KB at most)
-constexpr int EPI_THREADS = 128;
-constexpr int TMEM_COLS = 512;              // two 256-column fp32 accumulators (all of TMEM)
-constexpr int ACC_COLS = 256;
 
 struct ConvParams {
     const float *x;          // NHWC source, pixel stride xs floats
@@ -62,7 +59,8 @@ struct ConvParams {
                              //    stride-2 convolution: only even coordinates of the Hv x Wv virtual source are live)
     int Hv, Wv;              // virtual source dims seen by the conv (= Hs,Ws | 2Hs,2Ws | the stride-2 layer's input size)
     int Cin;                 // K channels per tap of ONE n-tile (grouped: the channel window, else all input channels)
-    int kwin;                // grouped / block-diagonal: n-tile nt reads input channels [nt*kwin, nt*kwin + Cin); 0 = dense
+    int kwin;                // grouped / block-diagonal: output channels c read the input-channel window
+                             //    [c / kwin * kwin, + kwin) (n_tile divides kwin); 0 = dense
     int KH, KW, stride, pad, dil;
     const float *wpack;      // packed weights (see pack kernel)
     int n_tile, n_tiles, Cout;
@@ -86,7 +84,6 @@ struct ConvParams {
     // stat_sum[c] += sum_p g*[bn(x)>0],  stat_sumsq[c] += sum_p g*[bn(x)>0]*xhat   (bts_bn_relu_bwd_reduce without its pass)
     int chunk_major;         // K order: k-block kb = (chunk kb / taps, tap kb % taps) -- consecutive k-blocks re-read the SAME
                              // pixels' lines shifted by one tap, so they hit in L1 instead of going to L2 nine times
-    int legacy;              // 1: round-1 single-lane MMA issue loop with separate A/B full barriers (fallback switch)
     int tma_adj;             // TMA mode: base-pixel coordinate = out*stride - tma_adj (the bounding box's lower corner)
     tc::FastDiv fd_taps;     // chunk-major: kb -> (kb / taps, kb % taps)
     tc::FastDiv fd_kc;       // TMA mode: k-block -> (tap, 32-channel chunk) = (kb / KC, kb % KC)
@@ -113,7 +110,8 @@ __device__ __forceinline__ void pack_one(const float *__restrict__ w, long long 
                                          float *__restrict__ wpack, int n_tile, int kwin, int cpg, int flags,
                                          long long idx) {
     // grouped (kwin > 0): Cin == Cout == total width, w is (width, cpg, KH, KW); rows = all channels, the K channels of
-    // n-tile nt are the window [nt*kwin, (nt+1)*kwin) and entries outside the row's group are zero (block diagonal)
+    // n-tile nt are the window of kwin channels that holds its rows (n_tile divides kwin) and entries outside the row's
+    // group are zero (block diagonal)
     const int Nrows = transpose_flip ? Cin : Cout;    // GEMM N
     const int Kch = kwin ? kwin : (transpose_flip ? Cout : Cin);      // GEMM K channels per tap
     const int CQ = (Kch + 3) / 4;
@@ -140,7 +138,7 @@ __device__ __forceinline__ void pack_one(const float *__restrict__ w, long long 
         bool live = true;
         int kc = ch, rr = row;            // K channel / row index into w's (co, ci) axes
         if (kwin) {
-            const int kglob = nt * kwin + ch;                 // global channel on the K side
+            const int kglob = nt * n_tile / kwin * kwin + ch;     // global channel on the K side
             live = (kglob / cpg) == (row / cpg);
             if (transpose_flip) { kc = kglob; rr = row % cpg; }   // w[co = kglob][ci_local = row % cpg]
             else { kc = kglob % cpg; }                            // w[co = row][ci_local = kglob % cpg]
@@ -200,41 +198,31 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackDesc 
 // ------------------------------------------------------------------------------------------- main kernel
 // dynamic smem, 1024-byte aligned base:
 //   [S stages][A_hi 16K | A_lo 16K | B_hi n_tile*128 | B_lo n_tile*128]   S = as many stages as fit (2..MAX_STAGES)
-//   [pre-op scale[KC*32], shift[KC*32]]  (PRE >= 2 only)   [mbarriers]
-// Narrow-N layers (n_tile <= 64: the DenseNet 3x3 convs, the full-resolution decoder convs, most dgrads) get 4-5
-// stages instead of 3: with two producer groups alternating k-blocks, 3 stages left each group at most one stage of
-// slack and the ncu samples showed the producers parked on `empty` 23 % of the time.
+//   [pre-op scale[KC*32], shift[KC*32]]  (PRE >= 2 only)   [mbarriers]   [epilogue statistics partials]
 constexpr int MAX_STAGES = 6;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in maximum per CTA
 constexpr int BAR_BYTES = 256;
-// per-CTA partial sums of the epilogue statistics: fp64, one private set per epilogue warp ([4][2][n_tile]) -- no atomics,
-// fixed accumulation order (round 2: the fp32 shared-memory atomics made a training step irreproducible at 3e-3 of the
-// gradient, tools/determinism_probe.py)
-constexpr int STAT_SETS = 4;
+// per-CTA partial sums of the epilogue statistics: fp64, one private set per consumer warp ([8][2][n_tile]) -- no atomics
+// inside the CTA and a fixed accumulation order, so a training step is reproducible run to run
+constexpr int STAT_SETS = CONSUMER_THREADS / 32;
 
 // PRE: 0 none, 1 ReLU, 2 affine, 3 affine + ReLU (compile-time so the per-element producer code carries no dead ops)
 // UP : nearest x2 up-sample folded into the address map;  VEC: 16-byte aligned rows (float4 loads)
 //
-// Index arithmetic (ncu, round 1: 84 % of the executed instructions were integer division sequences, predicate /
-// address recomputation and mbarrier spin loops -- each producer warp issued one instruction every ~9 cycles):
-//   * every k-block -> (tile, tap, channel chunk, stage, phase) mapping is carried in incrementally updated counters;
-//   * the per-tile pixel decode uses multiply-shift division by host-precomputed constants (FastDiv);
-//   * long waits (epilogue on the accumulator, weight loader on a free stage) back off with nanosleep so the spinning
-//     warps stop competing with the producers for issue slots.
+// Index arithmetic: every k-block -> (tile, tap, channel chunk, stage, phase) mapping is carried in incrementally updated
+// counters, and the per-tile pixel decode uses multiply-shift division by host-precomputed constants (FastDiv).
 // TMA = true: the activation tile is staged by the Tensor Memory Accelerator (one cp.async.bulk.tensor im2col load per
 // k-block lands 128 pixels x 32 channels, swizzled, zero-filled where the filter tap falls into the padding) and is used
 // AS IS as the A_hi operand (the tensor core reads the top 19 bits of each fp32 word); the producer warps only derive
 // A_lo = x - trunc_tf32(x) from shared memory (and apply the BN/ReLU pre-op in place) -- no global loads, no address /
-// bounds arithmetic, one shared store instead of two: ~2.8x fewer producer instructions per k-block.  K is enumerated per
-// tap in 32-channel chunks (identical to the dense-quad order whenever the K channels are a multiple of 32, which the
-// host requires), stride 1, no up-sample.
-// G: producer groups (4 warps each).  G = 2 keeps one k-block of register prefetch per thread (two F4[8] buffers).  G = 4
-// (narrow-N layers, where ncu showed the MMA warp waiting on `full` with the schedulers issuing on only 48% of the cycles
-// and two producer warps per scheduler stalled on their own dependency chains) drops the second buffer -- 4 producer warps
-// per scheduler, the other groups' work hides a group's load latency -- to fit 704 threads in the register file.
+// bounds arithmetic, one shared store instead of two.  K is enumerated per tap in 32-channel chunks (identical to the
+// dense-quad order whenever the K channels are a multiple of 32, which the host requires), stride 1, no up-sample.
+// G: producer groups (4 warps each).  G = 2 keeps one k-block of register prefetch per thread (two F4[8] buffers); G = 4
+// (narrow-N layers with >= 4 stages) drops the second buffer and lets the other groups' work hide a group's load latency.
 template <int PRE, int UP, bool VEC, bool TMA, int G>
-__global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap) {
-    constexpr int NUM_THREADS = 192 + 128 * G;
+__global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_kernel(const ConvParams p,
+                                                                                      const __grid_constant__ CUtensorMap tmap) {
+    constexpr int NUM_THREADS = CONSUMER_THREADS + 32 + 128 * G;
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-byte aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -245,21 +233,14 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + p.KC * 32;
     const uint32_t bar_off = pre_off + (PRE >= 2 ? (uint32_t)p.KC * 32u * 8u : 0u);
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + bar_off);
-    // bars: [0..MS) full (128 producer arrivals + the weight loader's expect_tx arrival + its bytes), [2MS..3MS) empty, then
-    // tmem_full[2], tmem_empty[2]; then the TMEM base word
+    // bars: [0..MS) full (128 producer arrivals [+ the weight loader's expect_tx arrival and its bytes]), [MS..2MS) raw
+    // (TMA mode: the activation tile and the weights land there), [2MS..3MS) empty (one arrival per consumer warp)
     const uint32_t bar0 = base + bar_off;
     auto full_a = [&](int s) { return bar0 + 8u * s; };
-    // ONE barrier per stage for the MMA warp (one try_wait per k-block).  TMA mode adds `raw` barriers for the loads:
-    // TMA bytes (A raw tile + weights) land on raw(s), the lo-producers wait there and then arrive on full(s).
     auto raw = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
-    const bool legacy = p.legacy != 0;
-    auto full_b = [&](int s) { return (TMA || legacy) ? raw(s) : full_a(s); };
+    auto full_b = [&](int s) { return TMA ? raw(s) : full_a(s); };
     auto empty = [&](int s) { return bar0 + 8u * (2 * MAX_STAGES + s); };
-    auto tmem_full = [&](int a) { return bar0 + 8u * (3 * MAX_STAGES + a); };
-    auto tmem_empty = [&](int a) { return bar0 + 8u * (3 * MAX_STAGES + 2 + a); };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 3 * MAX_STAGES + 4);
-    double *s_stat = reinterpret_cast<double *>(sm + bar_off + BAR_BYTES);    // [4 warps][2][n_tile], only when p.stat_sum
+    double *s_stat = reinterpret_cast<double *>(sm + bar_off + BAR_BYTES);    // [8 warps][2][n_tile], only when p.stat_sum
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int n_tile = p.n_tile;
@@ -272,29 +253,21 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
-            mbar_init(full_a(s), (TMA || legacy) ? PRODUCER_THREADS : PRODUCER_THREADS + 1);
+            mbar_init(full_a(s), TMA ? PRODUCER_THREADS : PRODUCER_THREADS + 1);
             mbar_init(raw(s), 1);
-            mbar_init(empty(s), 1);
-        }
-        for (int a = 0; a < 2; ++a) {
-            mbar_init(tmem_full(a), 1);
-            mbar_init(tmem_empty(a), EPI_THREADS);
+            mbar_init(empty(s), CONSUMER_THREADS / 32);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), TMEM_COLS);
     if (PRE >= 2) {
         for (int c = threadIdx.x; c < p.KC * 32; c += NUM_THREADS) {
             s_scale[c] = c < p.Cin ? p.pre_scale[c] : 0.f;
             s_shift[c] = c < p.Cin ? p.pre_shift[c] : 0.f;
         }
     }
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == LOADER_WARP) {
         // ===================== weight loader =====================
         if (lane == 0) {
             const uint32_t bytes = 2u * (uint32_t)n_tile * 128u;
@@ -306,6 +279,7 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
                 const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
                 const int nt = tile - (int)m_tile * p.n_tiles;
                 const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack) + (size_t)nt * KB * bytes;
+                const int win0 = p.kwin ? nt * n_tile / p.kwin * p.kwin : 0;     // grouped: first channel of the K window
                 int tw = 0, th = 0, tn = 0;
                 if (TMA) {                         // first output pixel of the tile -> base-pixel coordinate of the im2col walk
                     const uint32_t m0 = m_tile * BLOCK_M;
@@ -321,7 +295,7 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
                     if (TMA) {
                         mbar_arrive_expect_tx(raw(s), bytes + (uint32_t)A_TILE_BYTES);
                         const int ky = (int)fdiv((uint32_t)tap, p.fd_kw), kx = tap - ky * p.KW;
-                        tma_im2col_4d(base + (uint32_t)s * stage_bytes, &tmap, nt * p.kwin + kc * 32, tw, th, tn, raw(s),
+                        tma_im2col_4d(base + (uint32_t)s * stage_bytes, &tmap, win0 + kc * 32, tw, th, tn, raw(s),
                                       (uint16_t)(kx * p.dil), (uint16_t)(ky * p.dil));
                         if (++kc == p.KC) { kc = 0; ++tap; }
                     } else {
@@ -332,131 +306,9 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
                 }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // Instruction-count economy, part 2 (round 2; ncu source view of the round-1 kernel, profiles/r01_conv_db1_3x3_v4):
-        // the issuing warp executed ~300 instructions per k-block -- two try_waits, four 64-bit descriptors rebuilt from
-        // addresses, per-MMA predicate set-up and the ELECT / BRA.U.ANY uniformity loops the compiler wraps around every
-        // uniform-datapath instruction inside a divergent `if (lane == 0)` -- at ~4 cycles each: ~1300 cycles per k-block
-        // WHATEVER N is; the tensor pipe itself was busy 39 cycles per MMA (= N/256 * 128, the hardware floor).  Hence:
-        //   * the whole warp runs the loop (warp-uniform control flow), one elected lane issues;
-        //   * one `full` barrier per stage; descriptors advance by adding constants to stage-0 descriptors;
-        //   * the precision / stacking mode is resolved outside the tile loop.
-        // MMA count economy of round 1 is kept: n_tile <= 128 -> A_hi*[B_hi;B_lo] is ONE instruction of width 2*n_tile
-        // (+ A_lo*B_hi): 2 MMAs per k-step; wider tiles: 3 MMAs per k-step over one 256-wide tile.
-        if (legacy) {
-            // ---- round-1 issue loop, kept verbatim as a fallback (bts_conv_set_issue_mode(0)): single lane, two barriers
-        if (lane == 0 && !TMA) {
-            // Instruction-count economy (measured, round 1): a tcgen05.mma with M=128, K=8 (tf32) costs ~115-130 cycles
-            // whatever N is -- fetching the 128 A rows from shared memory sets the pace -- so every layer ran at ~1400
-            // cycles per k-block (12 MMAs) regardless of Cout, load latency or producer instruction count.  Hence:
-            //   * n_tile <= 128: B_hi and B_lo are adjacent in the stage, so ONE instruction with N = 2*n_tile computes
-            //     A_hi*[B_hi;B_lo] into 2*n_tile accumulator columns (the epilogue adds the two halves); the third
-            //     product A_lo*B_hi is a second instruction: 2 MMAs per k-step instead of 3;
-            //   * n_tile <= 256 is one tile (3 MMAs per k-step, the activation tile produced once) instead of two tiles.
-            const bool stack = n_tile <= 128;
-            const uint32_t idesc = make_idesc(BLOCK_M, n_tile);
-            const uint32_t idesc2 = make_idesc(BLOCK_M, 2 * n_tile);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int ti = 0; ti < my_tiles; ++ti) {
-                const int acc = ti & 1;
-                const uint32_t d_tmem = tmem_base + (uint32_t)(acc * ACC_COLS);
-                mbar_wait(tmem_empty(acc), (uint32_t)((ti >> 1) & 1) ^ 1);     // epilogue has drained this accumulator
-                tc_fence_after();
-                for (int kb = 0; kb < KB; ++kb) {
-                    mbar_wait(full_a(s), ph);
-                    mbar_wait(full_b(s), ph);
-                    tc_fence_after();
-                    const uint32_t a_hi = base + (uint32_t)s * stage_bytes;
-                    const uint32_t a_lo = a_hi + A_TILE_BYTES;
-                    const uint32_t b_hi = a_hi + 2 * A_TILE_BYTES;
-                    const uint32_t b_lo = b_hi + n_tile * 128;
-                    const uint64_t dah = make_desc(a_hi), dal = make_desc(a_lo), dbh = make_desc(b_hi), dbl = make_desc(b_lo);
-                    if (p.precision == 0) {
-                        if (stack) {
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 8; ++k) {
-                                umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc2, (kb | k) != 0);   // A_hi * [B_hi ; B_lo]
-                                umma_tf32(d_tmem, dal + 2 * k, dbh + 2 * k, idesc, 1);                // A_lo * B_hi
-                            }
-                        } else {
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 8; ++k)   // small cross terms first
-                                umma_tf32(d_tmem, dal + 2 * k, dbh + 2 * k, idesc, (kb | k) != 0);
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dah + 2 * k, dbl + 2 * k, idesc, 1);
-#pragma unroll
-                            for (int k = 0; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc, 1);
-                        }
-                    } else {
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / 8; ++k)
-                            umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc, (kb | k) != 0);
-                    }
-                    umma_commit(empty(s));       // frees the stage when these MMAs have read it
-                    if (++s == S) { s = 0; ph ^= 1; }
-                }
-                umma_commit(tmem_full(acc));     // accumulator of this tile complete
-            }
-        }
-        } else {
-        const bool stack = n_tile <= 128;
-        const uint32_t idesc = make_idesc(BLOCK_M, n_tile);
-        const uint32_t idesc2 = make_idesc(BLOCK_M, 2 * n_tile);
-        const uint64_t dA0 = make_desc(base);                                  // A_hi of stage 0
-        const uint64_t oAlo = (uint64_t)(A_TILE_BYTES >> 4), oBhi = (uint64_t)((2 * A_TILE_BYTES) >> 4);
-        const uint64_t oBlo = oBhi + (uint64_t)((n_tile * 128) >> 4), stage_step = (uint64_t)(stage_bytes >> 4);
-        const int mode = p.precision != 0 ? 2 : (stack ? 0 : 1);
-        const bool leader = elect_one();
-        int s = 0;
-        uint32_t ph = 0;
-        uint64_t d = dA0;
-        uint32_t bfull = full_a(0), bempty = empty(0);
-        for (int ti = 0; ti < my_tiles; ++ti) {
-            const int acc = ti & 1;
-            const uint32_t d_tmem = tmem_base + (uint32_t)(acc * ACC_COLS);
-            mbar_wait(tmem_empty(acc), (uint32_t)((ti >> 1) & 1) ^ 1);     // epilogue has drained this accumulator
-            tc_fence_after();
-            for (int kb = 0; kb < KB; ++kb) {
-                mbar_wait(bfull, ph);
-                tc_fence_after();
-                if (leader) {
-                    const uint64_t dah = d, dal = d + oAlo, dbh = d + oBhi, dbl = d + oBlo;
-                    const uint32_t first = kb != 0;
-                    if (mode == 0) {
-                        umma_tf32(d_tmem, dah, dbh, idesc2, first);          // A_hi * [B_hi ; B_lo]
-                        umma_tf32(d_tmem, dal, dbh, idesc, 1);               // A_lo * B_hi
-#pragma unroll
-                        for (int k = 1; k < BLOCK_K / 8; ++k) {
-                            umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc2, 1);
-                            umma_tf32(d_tmem, dal + 2 * k, dbh + 2 * k, idesc, 1);
-                        }
-                    } else if (mode == 1) {
-                        umma_tf32(d_tmem, dal, dbh, idesc, first);           // small cross terms first
-#pragma unroll
-                        for (int k = 1; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dal + 2 * k, dbh + 2 * k, idesc, 1);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dah + 2 * k, dbl + 2 * k, idesc, 1);
-#pragma unroll
-                        for (int k = 0; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc, 1);
-                    } else {
-                        umma_tf32(d_tmem, dah, dbh, idesc, first);
-#pragma unroll
-                        for (int k = 1; k < BLOCK_K / 8; ++k) umma_tf32(d_tmem, dah + 2 * k, dbh + 2 * k, idesc, 1);
-                    }
-                    umma_commit(bempty);         // frees the stage when these MMAs have read it
-                    if (kb == KB - 1) umma_commit(tmem_full(acc));     // accumulator of this tile complete
-                }
-                __syncwarp();
-                d += stage_step; bfull += 8u; bempty += 8u;
-                if (++s == S) { s = 0; ph ^= 1; d = dA0; bfull = full_a(0); bempty = empty(0); }
-            }
-        }
-        }   // lean issue loop
-    } else if (warp < 2 + 4 * G) {
+    } else if (warp > LOADER_WARP) {
         // ===================== activation producers (G groups x 4 warps) =====================
-        const int pt = threadIdx.x - 64;           // 0..255
+        const int pt = threadIdx.x - (CONSUMER_THREADS + 32);
         const int grp = pt >> 7;                   // producer group: global k-blocks gk == grp (mod G)
         const int t = pt & 127;
         const int chunk = t & 7;                   // 16-byte chunk of the 128-byte row
@@ -556,7 +408,8 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
             const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
             const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
             const uint32_t m_base = m_tile * BLOCK_M + (uint32_t)r0;
-            const int cwin = (tile - (int)m_tile * p.n_tiles) * p.kwin;     // first input channel of this n-tile's window
+            const int nt = tile - (int)m_tile * p.n_tiles;
+            const int cwin = p.kwin ? nt * p.n_tile / p.kwin * p.kwin : 0;     // first input channel of this n-tile's window
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const uint32_t m = m_base + 16u * i;
@@ -703,158 +556,167 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
         }
         }   // !TMA
     } else {
-        // ===================== epilogue warps (the last four) =====================
-        const int q = warp & 3;                                  // TMEM lane quarter this warp may access
-        const int row = q * 32 + lane;
-        const bool ovec = ((p.os & 3) == 0) && ((((uintptr_t)p.out) & 15) == 0);
-        for (int ti = 0; ti < my_tiles; ++ti) {
-            const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-            const int m_tile = (int)fdiv((uint32_t)tile, p.fd_ntiles), nt = tile - m_tile * p.n_tiles;
-            const int acc = ti & 1;
-            const long long m = (long long)m_tile * BLOCK_M + row;
-            float *orow = p.out + (m < p.M ? m : 0) * p.os + (long long)nt * n_tile;
-            mbar_wait_sleep(tmem_full(acc), (uint32_t)((ti >> 1) & 1));
-            tc_fence_after();
-            const uint32_t t_addr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * ACC_COLS);
-            const bool stack = n_tile <= 128 && p.precision == 0;   // columns [n_tile, 2 n_tile) hold A_hi * B_lo
-            for (int cc = 0; cc < n_tile; cc += 16) {
-                uint32_t r[16];
-                tmem_ld8(t_addr + (uint32_t)cc, reinterpret_cast<uint32_t(&)[8]>(r[0]));
-                tmem_ld8(t_addr + (uint32_t)cc + 8, reinterpret_cast<uint32_t(&)[8]>(r[8]));
-                if (stack) {
-                    uint32_t r2[16];
-                    tmem_ld8(t_addr + (uint32_t)(n_tile + cc), reinterpret_cast<uint32_t(&)[8]>(r2[0]));
-                    tmem_ld8(t_addr + (uint32_t)(n_tile + cc) + 8, reinterpret_cast<uint32_t(&)[8]>(r2[8]));
-                    tmem_ld_wait();
+        // ===================== consumers: two warpgroups, rows [64 wg, 64 wg + 64) of every 128-pixel tile =========
+        // 3xTF32: per k8 step A_lo*B_hi, A_hi*B_lo, A_hi*B_hi (small cross terms first).  The tensor cores accumulate one
+        // k-block (4 k8 steps x 3 products) into `acc`; it is then added into the fp32 tile sum `tot` with round-to-nearest
+        // adds, which keeps the accumulation error of long-K layers at the level of a plain fp32 sum.  The stage is handed
+        // back to the loader / producers as soon as its wgmma group has completed.
+        const int wg = warp >> 2;
+        const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // rows row and row + 8 of the tile
+        const int cq = (lane & 3) * 2;                               // columns 8 j + cq, 8 j + cq + 1
+        const bool ovec = ((p.os & 1) == 0) && ((((uintptr_t)p.out) & 7) == 0);
+        const bool single = p.precision != 0;
+        auto consume = [&](auto NT) {
+            constexpr int N = decltype(NT)::value;
+            constexpr int R = N / 2;
+            float acc[R], tot[R];
+            const uint64_t dA0 = make_desc(base + (uint32_t)wg * (64u * 128u));      // A_hi of stage 0, this warpgroup's rows
+            const uint64_t oAlo = (uint64_t)(A_TILE_BYTES >> 4);
+            const uint64_t oBhi = (uint64_t)((2 * A_TILE_BYTES - wg * 64 * 128) >> 4);
+            const uint64_t oBlo = oBhi + (uint64_t)((N * 128) >> 4), stage_step = (uint64_t)(stage_bytes >> 4);
+            int s = 0;
+            uint32_t ph = 0;
+            uint64_t d = dA0;
+            for (int ti = 0; ti < my_tiles; ++ti) {
+                const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+                const int m_tile = (int)fdiv((uint32_t)tile, p.fd_ntiles), nt = tile - m_tile * p.n_tiles;
 #pragma unroll
-                    for (int e = 0; e < 16; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-                } else {
-                    tmem_ld_wait();
+                for (int i = 0; i < R; ++i) tot[i] = 0.f;
+                for (int kb = 0; kb < KB; ++kb) {
+                    mbar_wait(full_a(s), ph);
+                    wgmma_fence();
+                    const uint64_t dah = d, dal = d + oAlo, dbh = d + oBhi, dbl = d + oBlo;
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / 8; ++k) {
+                        const uint32_t accumulate = k != 0;
+                        if (single) {
+                            Wgmma<N>::mma(acc, dah + 2 * k, dbh + 2 * k, accumulate);
+                        } else {
+                            Wgmma<N>::mma(acc, dal + 2 * k, dbh + 2 * k, accumulate);
+                            Wgmma<N>::mma(acc, dah + 2 * k, dbl + 2 * k, 1);
+                            Wgmma<N>::mma(acc, dah + 2 * k, dbh + 2 * k, 1);
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_operands(acc);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(empty(s));
+#pragma unroll
+                    for (int i = 0; i < R; ++i) tot[i] += acc[i];
+                    d += stage_step;
+                    if (++s == S) { s = 0; ph ^= 1; d = dA0; }
                 }
-                if (m < p.M) {
-                    const int cbase = nt * n_tile + cc;          // absolute output channel
+
+                // ---- epilogue straight from the accumulator registers
+                const long long m0 = (long long)m_tile * BLOCK_M + row, m1 = m0 + 8;
+                float *orow0 = p.out + (m0 < p.M ? m0 : 0) * p.os + (long long)nt * n_tile;
+                float *orow1 = p.out + (m1 < p.M ? m1 : 0) * p.os + (long long)nt * n_tile;
 #pragma unroll
-                    for (int e4 = 0; e4 < 16; e4 += 4) {
-                        float o[4];
+                for (int j = 0; j < N / 8; ++j) {
+                    const int col = 8 * j + cq;
+                    const int cabs = nt * n_tile + col;
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float a = __uint_as_float(r[e4 + e]);
+                    for (int i = 0; i < 2; ++i) {
+                        float o[2];
+#pragma unroll
+                        for (int c = 0; c < 2; ++c) {
+                            float a = tot[4 * j + 2 * i + c];
                             if (p.act == 1) a = a > 0.f ? a : expm1f(a);
                             else if (p.act == 2) a = 1.0f / (1.0f + expf(-a));
-                            o[e] = a;
+                            o[c] = a;
                         }
-                        if (ovec && cbase + e4 + 3 < p.Cout) {
-                            *reinterpret_cast<float4 *>(orow + cc + e4) = make_float4(o[0], o[1], o[2], o[3]);
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (cbase + e4 + e < p.Cout) orow[cc + e4 + e] = o[e];
+                        if ((i ? m1 : m0) < p.M) {
+                            float *orow = i ? orow1 : orow0;
+                            if (ovec && cabs + 1 < p.Cout) {
+                                *reinterpret_cast<float2 *>(orow + col) = make_float2(o[0], o[1]);
+                            } else {
+                                if (cabs < p.Cout) orow[col] = o[0];
+                                if (cabs + 1 < p.Cout) orow[col + 1] = o[1];
+                            }
                         }
                     }
                 }
                 if (p.stat_sum) {
-                    // BatchNorm batch statistics of the tensor being produced (bts_bn_stats fused into its producer):
-                    // column sums over the warp's 32 rows by a transposing butterfly (16 shuffles per quantity instead
-                    // of 80), then shared-memory partials per CTA; flushed with fp64 atomics below.
+                    // BatchNorm batch statistics of the tensor being produced (bts_bn_stats fused into its producer): column
+                    // sums over the warp's 16 rows by a butterfly over the 8 row lanes, then per-warp fp64 partials per CTA.
                     // (host guarantees act == none here: the statistics are those of the raw conv output)
                     // With bnb_x set the two quantities are instead the BatchNorm-BACKWARD sums of the gradient tile.
-                    float s1[16], s2[16];
-                    if (p.bnb_x) {
-                        const int cb0 = nt * n_tile + cc;
-                        const float *xr = p.bnb_x + (m < p.M ? m : 0) * p.bnb_xs + cb0;
-                        const bool xvec = ((p.bnb_xs & 3) == 0) && ((((uintptr_t)p.bnb_x) & 15) == 0) && cb0 + 15 < p.Cout &&
-                                          ((p.Cout & 3) == 0);
 #pragma unroll
-                        for (int e4 = 0; e4 < 16; e4 += 4) {
-                            float xv[4], sc[4], sh[4], mu[4], is[4];
-                            if (xvec) {
-                                const float4 q4 = m < p.M ? __ldg(reinterpret_cast<const float4 *>(xr + e4)) : make_float4(0.f, 0.f, 0.f, 0.f);
-                                const float4 a4 = __ldg(reinterpret_cast<const float4 *>(p.bnb_st + cb0 + e4));
-                                const float4 b4 = __ldg(reinterpret_cast<const float4 *>(p.bnb_st + p.Cout + cb0 + e4));
-                                const float4 c4 = __ldg(reinterpret_cast<const float4 *>(p.bnb_st + 2 * p.Cout + cb0 + e4));
-                                const float4 d4 = __ldg(reinterpret_cast<const float4 *>(p.bnb_st + 3 * p.Cout + cb0 + e4));
-                                xv[0] = q4.x; xv[1] = q4.y; xv[2] = q4.z; xv[3] = q4.w;
-                                sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
-                                sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
-                                mu[0] = c4.x; mu[1] = c4.y; mu[2] = c4.z; mu[3] = c4.w;
-                                is[0] = d4.x; is[1] = d4.y; is[2] = d4.z; is[3] = d4.w;
-                            } else {
+                    for (int j = 0; j < N / 8; ++j) {
+                        const int col = 8 * j + cq;
+                        const int cabs = nt * n_tile + col;
 #pragma unroll
-                                for (int e = 0; e < 4; ++e) {
-                                    const int c = cb0 + e4 + e;
-                                    const bool ok = c < p.Cout;
-                                    const int ce = ok ? c : p.Cout - 1;
-                                    xv[e] = (ok && m < p.M) ? __ldg(xr + e4 + e) : 0.f;
-                                    sc[e] = __ldg(p.bnb_st + ce); sh[e] = __ldg(p.bnb_st + p.Cout + ce);
-                                    mu[e] = __ldg(p.bnb_st + 2 * p.Cout + ce); is[e] = __ldg(p.bnb_st + 3 * p.Cout + ce);
+                        for (int c = 0; c < 2; ++c) {
+                            float s1 = 0.f, s2 = 0.f;
+                            const int ch = cabs + c;
+#pragma unroll
+                            for (int i = 0; i < 2; ++i) {
+                                const long long m = i ? m1 : m0;
+                                if (m < p.M && ch < p.Cout) {
+                                    const float g = tot[4 * j + 2 * i + c];
+                                    if (p.bnb_x) {
+                                        const float xv = __ldg(p.bnb_x + m * p.bnb_xs + ch);
+                                        const float sc = __ldg(p.bnb_st + ch), sh = __ldg(p.bnb_st + p.Cout + ch);
+                                        const float mu = __ldg(p.bnb_st + 2 * p.Cout + ch), is = __ldg(p.bnb_st + 3 * p.Cout + ch);
+                                        const float y = fmaf(xv, sc, sh);
+                                        const float gm = (!p.bnb_relu || y > 0.f) ? g : 0.f;
+                                        s1 += gm;
+                                        s2 += gm * ((xv - mu) * is);
+                                    } else {
+                                        s1 += g;
+                                        s2 += g * g;
+                                    }
                                 }
                             }
 #pragma unroll
-                            for (int e = 0; e < 4; ++e) {
-                                const float gval = m < p.M ? __uint_as_float(r[e4 + e]) : 0.f;
-                                const float y = fmaf(xv[e], sc[e], sh[e]);
-                                const float gm = (!p.bnb_relu || y > 0.f) ? gval : 0.f;
-                                s1[e4 + e] = gm;
-                                s2[e4 + e] = gm * ((xv[e] - mu[e]) * is[e]);
+                            for (int w = 4; w <= 16; w <<= 1) {
+                                s1 += __shfl_xor_sync(0xffffffffu, s1, w);
+                                s2 += __shfl_xor_sync(0xffffffffu, s2, w);
+                            }
+                            if (lane < 4 && ch < p.Cout) {                 // this (warp, lane) owns the slot: plain adds
+                                double *mine = s_stat + (size_t)warp * 2 * n_tile;
+                                mine[col + c] += (double)s1;
+                                mine[n_tile + col + c] += (double)s2;
                             }
                         }
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 16; ++e) {
-                            const float a = m < p.M ? __uint_as_float(r[e]) : 0.f;
-                            s1[e] = a;
-                            s2[e] = a * a;
-                        }
-                    }
-#pragma unroll
-                    for (int w = 8; w >= 1; w >>= 1) {            // lane mask 16, 8, 4, 2 <-> keep 8, 4, 2, 1 columns
-                        const bool upper = (lane & (2 * w)) != 0;
-#pragma unroll
-                        for (int j = 0; j < w; ++j) {
-                            const float k1 = upper ? s1[w + j] : s1[j], d1 = upper ? s1[j] : s1[w + j];
-                            const float k2 = upper ? s2[w + j] : s2[j], d2 = upper ? s2[j] : s2[w + j];
-                            s1[j] = k1 + __shfl_xor_sync(0xffffffffu, d1, 2 * w);
-                            s2[j] = k2 + __shfl_xor_sync(0xffffffffu, d2, 2 * w);
-                        }
-                    }
-                    s1[0] += __shfl_xor_sync(0xffffffffu, s1[0], 1);
-                    s2[0] += __shfl_xor_sync(0xffffffffu, s2[0], 1);
-                    const int col = cc + (lane >> 1);             // lane bits 4..1 = column within the 16-column group
-                    if ((lane & 1) == 0 && nt * n_tile + col < p.Cout) {       // this (warp, lane) owns the slot: plain adds
-                        double *mine = s_stat + (size_t)q * 2 * n_tile;
-                        mine[col] += (double)s1[0];
-                        mine[n_tile + col] += (double)s2[0];
                     }
                 }
-            }
-            if (p.stat_sum && p.n_tiles > 1) {
-                // several N tiles per layer (1x1 dgrads onto wide slabs): the per-CTA partials belong to THIS tile's channel
-                // range -- flush them before the next tile (four epilogue warps only)
-                asm volatile("bar.sync 1, 128;" ::: "memory");
-                for (int c = (int)threadIdx.x - (NUM_THREADS - EPI_THREADS); c < n_tile; c += EPI_THREADS) {
-                    const int ch = nt * n_tile + c;
-                    double t1 = 0.0, t2 = 0.0;
-                    for (int w = 0; w < STAT_SETS; ++w) {                // fixed order over the four warps
-                        t1 += s_stat[(size_t)w * 2 * n_tile + c];
-                        t2 += s_stat[(size_t)w * 2 * n_tile + n_tile + c];
-                        s_stat[(size_t)w * 2 * n_tile + c] = 0.0;
-                        s_stat[(size_t)w * 2 * n_tile + n_tile + c] = 0.0;
+                if (p.stat_sum && p.n_tiles > 1) {
+                    // several N tiles per layer: the per-CTA partials belong to THIS tile's channel range -- flush them
+                    // before the next tile (consumer warps only)
+                    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");
+                    for (int c = (int)threadIdx.x; c < n_tile; c += CONSUMER_THREADS) {
+                        const int ch = nt * n_tile + c;
+                        double t1 = 0.0, t2 = 0.0;
+                        for (int w = 0; w < STAT_SETS; ++w) {                // fixed order over the consumer warps
+                            t1 += s_stat[(size_t)w * 2 * n_tile + c];
+                            t2 += s_stat[(size_t)w * 2 * n_tile + n_tile + c];
+                            s_stat[(size_t)w * 2 * n_tile + c] = 0.0;
+                            s_stat[(size_t)w * 2 * n_tile + n_tile + c] = 0.0;
+                        }
+                        if (ch < p.Cout) {
+                            atomicAdd(p.stat_sum + ch, t1);
+                            atomicAdd(p.stat_sumsq + ch, t2);
+                        }
                     }
-                    if (ch < p.Cout) {
-                        atomicAdd(p.stat_sum + ch, t1);
-                        atomicAdd(p.stat_sumsq + ch, t2);
-                    }
+                    asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");
                 }
-                asm volatile("bar.sync 1, 128;" ::: "memory");
             }
-            tc_fence_before();
-            mbar_arrive(tmem_empty(acc));        // this thread is done reading the accumulator
+        };
+        switch (n_tile) {
+            case 16: consume(std::integral_constant<int, 16>()); break;
+            case 32: consume(std::integral_constant<int, 32>()); break;
+            case 48: consume(std::integral_constant<int, 48>()); break;
+            default:
+                if constexpr (G == 2) consume(std::integral_constant<int, 64>());   // four groups run n_tile <= 48 only
+                break;
         }
         if (p.stat_sum && p.n_tiles == 1) {
-            asm volatile("bar.sync 1, 128;" ::: "memory");       // the four epilogue warps only
-            for (int c = (int)threadIdx.x - (NUM_THREADS - EPI_THREADS); c < p.Cout; c += EPI_THREADS) {
+            asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");
+            for (int c = (int)threadIdx.x; c < p.Cout; c += CONSUMER_THREADS) {
                 double t1 = 0.0, t2 = 0.0;
-                for (int w = 0; w < STAT_SETS; ++w) {                    // fixed order over the four warps
+                for (int w = 0; w < STAT_SETS; ++w) {                    // fixed order over the consumer warps
                     t1 += s_stat[(size_t)w * 2 * n_tile + c];
                     t2 += s_stat[(size_t)w * 2 * n_tile + n_tile + c];
                 }
@@ -863,9 +725,6 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
             }
         }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, TMEM_COLS);
 }
 
 
@@ -875,7 +734,7 @@ __global__ void __launch_bounds__(192 + 128 * G, 1) conv_tc_kernel(const ConvPar
 extern "C" int bts_conv_n_tile(int Cout) {
     int n = (Cout + 15) / 16 * 16;
     if (n > MAX_N) {
-        // split into equal tiles <= 256, multiples of 16
+        // split into equal tiles <= MAX_N, multiples of 16
         const int tiles = (n + MAX_N - 1) / MAX_N;
         n = ((Cout + tiles - 1) / tiles + 15) / 16 * 16;
     }
@@ -910,8 +769,9 @@ extern "C" int bts_conv_pack_weights(const float *w, long long s_co, long long s
 }
 
 // Grouped convolution whose groups tile a 128-wide diagonal block (ResNeXt 3x3: width % kwin == 0, kwin % cpg == 0):
-// w is (width, cpg, KH, KW); the packed operator has width/kwin n-tiles of kwin rows, each over the K window of kwin
-// channels -- zeros outside the row's group.  Run with bts_conv_fwd_ex(kwin = bts_conv_group_window(width, cpg)).
+// w is (width, cpg, KH, KW); the packed operator has width/n_tile n-tiles of n_tile = bts_conv_group_n_tile(kwin) rows,
+// each over the K window of kwin channels that holds its rows -- zeros outside the row's group.  Run with
+// bts_conv_fwd_ex(kwin = bts_conv_group_window(width, cpg)).
 extern "C" int bts_conv_group_window(int width, int cpg) {
     if (width < 1 || cpg < 1 || width % cpg) return 0;
     int k = 128;
@@ -924,12 +784,21 @@ extern "C" int bts_conv_group_window(int width, int cpg) {
     return k;
 }
 
+// n-tile width of a grouped operator: the widest multiple of 16 <= MAX_N that divides the window
+extern "C" int bts_conv_group_n_tile(int kwin) {
+    if (kwin < 16 || kwin % 16) return 0;
+    int n = MAX_N;
+    while (kwin % n) n -= 16;
+    return n;
+}
+
 extern "C" long long bts_conv_packed_floats_grouped(int width, int cpg, int KH, int KW) {
     const int kwin = bts_conv_group_window(width, cpg);
     if (!kwin) return 0;
     const int CQ = kwin / 4;
     const int KB = (KH * KW * CQ + 7) / 8;
-    return (long long)(width / kwin) * KB * 2 * kwin * 32;
+    const int nt = bts_conv_group_n_tile(kwin);
+    return (long long)(width / nt) * KB * 2 * nt * 32;
 }
 
 extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw,
@@ -944,15 +813,14 @@ extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, lon
     const long long cap = (long long)bts_num_sms() * 16;
     if (grid > cap) grid = cap;
     pack_weights_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(w, s_co, s_ci, s_kh, s_kw, width, width, KH, KW,
-                                                                    transpose_flip, wpack, kwin, width / kwin, kwin, cpg, flags);
+                                                                    transpose_flip, wpack, bts_conv_group_n_tile(kwin),
+                                                                    width / bts_conv_group_n_tile(kwin), kwin, cpg, flags);
     BTS_LAUNCH_CHECK();
     return 0;
 }
 
 // ---- TMA tensor map of the NHWC activation tensor, im2col mode (cuTensorMapEncodeIm2col through the runtime's driver
 //      entry-point query: no link-time dependency on libcuda)
-static int g_issue_legacy = 0;  // 1: round-1 MMA issue loops in conv_tc / wgrad_tc / wgrad2_tc (fallback switch)
-int bts_issue_legacy() { return g_issue_legacy; }
 static int g_producer_groups = 0;   // 0 / 4: four groups where the ring has >= 4 stages, 2: always two
 static int g_tma_mode = 0;      // 0 off, 1 on, 2 on with base-pixel coordinates NOT shifted by the lower corner, 3 on + strict
 
@@ -1003,11 +871,6 @@ extern "C" int bts_conv_set_producer_groups(int g) {
     return 0;
 }
 
-// 1 (default): lean whole-warp MMA issue loops; 0: the round-1 single-lane loops (kept as a fallback switch for bring-up)
-extern "C" int bts_conv_set_issue_mode(int lean) {
-    g_issue_legacy = lean ? 0 : 1;
-    return 0;
-}
 
 struct BnBwdArgs {
     const float *x; long long xs; const float *st; int relu;
@@ -1027,7 +890,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     if (act < 0 || act > 2 || precision < 0 || precision > 1) return BTS_EINVAL;
     if (upsample2 < 0 || upsample2 > 2 || kwin < 0) return BTS_EINVAL;
     if (upsample2 == 2 && (stride != 1 || out_h < 1 || out_w < 1)) return BTS_EINVAL;
-    if (kwin && (pre_scale || Cin % kwin || Cout % kwin)) return BTS_EINVAL;   // window = n-tile width; no pre-op on grouped convs
+    if (kwin && (pre_scale || Cin % kwin || Cout % kwin)) return BTS_EINVAL;   // whole windows; no pre-op on grouped convs
     if (!bts_aligned16(wpack)) return BTS_EALIGN;
     if (B == 0) return 0;
     if ((long long)B * Hs * Ws * x_pixel_stride >= 0x7fffffffLL) return BTS_EINVAL;   // 32-bit element offsets
@@ -1036,8 +899,8 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.kwin = kwin;
     p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad; p.dil = dil;
     p.wpack = wpack; p.Cout = Cout;
-    p.n_tile = kwin ? kwin : bts_conv_n_tile(Cout);
-    if (kwin && (kwin % 16 || kwin > MAX_N)) return BTS_EINVAL;
+    if (kwin % 16) return BTS_EINVAL;
+    p.n_tile = kwin ? bts_conv_group_n_tile(kwin) : bts_conv_n_tile(Cout);
     p.n_tiles = (Cout + p.n_tile - 1) / p.n_tile;
     p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu ? 1 : 0;
     p.out = out; p.os = out_pixel_stride; p.act = act; p.precision = precision;
@@ -1049,7 +912,6 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
         p.bnb_x = bnb->x; p.bnb_xs = bnb->xs; p.bnb_st = bnb->st; p.bnb_relu = bnb->relu ? 1 : 0;
     }
     if (stat_sum && act != 0) return BTS_EINVAL;                        // statistics of the raw conv output only
-    if (stat_sum && !bnb && p.n_tiles != 1) return BTS_EINVAL;          // forward statistics: one N tile (Cout <= 256)
     const int Hin = p.up ? 2 * Hs : Hs, Win = p.up ? 2 * Ws : Ws;
     p.Hv = Hin; p.Wv = Win;      // mode 2: live source coordinates are the even ones below 2Hs x 2Ws, zeros everywhere else
     p.Hout = p.up == 2 ? out_h : (Hin + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
@@ -1092,10 +954,9 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     memset(&tmap, 0, sizeof(tmap));
     bool use_tma = false;
     p.tma_adj = 0;
-    p.legacy = g_issue_legacy;
     p.fd_taps = make_fastdiv((uint32_t)(KH * KW));
     p.fd_kc = make_fastdiv((uint32_t)p.KC);
-    if (g_tma_mode != 0 && !g_issue_legacy && !p.chunk_major && p.up == 0 && stride == 1 && p.vec_ok && (p.Cin % 32) == 0 && pad <= 127 &&
+    if (g_tma_mode != 0 && !p.chunk_major && p.up == 0 && stride == 1 && p.vec_ok && (p.Cin % 32) == 0 && pad <= 127 &&
         dil * (KH - 1) - pad <= 128 && dil * (KW - 1) - pad <= 128 && dil * (KH - 1) <= 255 && dil * (KW - 1) <= 255) {
         const int rc = make_im2col_map(&tmap, x, x_pixel_stride, B, Hs, Ws, kwin ? Cin : p.Cin, KH, KW, pad, dil);
         if (rc == 0) {
@@ -1105,10 +966,9 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
             return rc;                                   // forced: report why the map could not be built
         }
     }
-    // four producer groups wherever the ring has >= 4 stages for them to work concurrently (i.e. every layer but the
-    // 256-wide tiles, which are tensor-bound anyway).  Measured on B200 (profiles/r02_producer_groups.txt): dense 3x3
-    // 192->48 457 -> 393 us, 161->64 1.38 -> 1.22 ms, never slower; K16 step 99.4 -> 97.4 ms.
-    const bool four = !use_tma && !g_issue_legacy && p.stages >= 4 && g_producer_groups != 2;
+    // four producer groups on the narrow layers (n_tile <= 48), where producing the activation tile, not the tensor
+    // cores, sets the k-block time; the 800-thread CTA leaves no registers for a wider accumulator
+    const bool four = !use_tma && p.stages >= 4 && p.n_tile <= FOUR_GROUPS_MAX_N && g_producer_groups != 2;
 #define BTS_LAUNCH_G(PRE, UP, VEC, TMA, G)                                                                         \
     do {                                                                                                           \
         static bool attr_set_[BTS_MAX_DEVICES] = {};                                                               \
@@ -1119,7 +979,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
             if (err != cudaSuccess) return (int)err;                                                               \
             attr_set = true;                                                                                       \
         }                                                                                                          \
-        conv_tc_kernel<PRE, UP, VEC, TMA, G><<<grid, 192 + 128 * G, smem, (cudaStream_t)stream>>>(p, tmap);         \
+        conv_tc_kernel<PRE, UP, VEC, TMA, G><<<grid, CONSUMER_THREADS + 32 + 128 * G, smem, (cudaStream_t)stream>>>(p, tmap);         \
     } while (0)
 #define BTS_LAUNCH(PRE, UP, VEC, TMA)                                                                              \
     do {                                                                                                           \

@@ -1,6 +1,6 @@
 // Streaming NHWC kernels that replace the ATen/cuDNN glue of the BTS decoder and encoder transitions (reference
 // pytorch/bts.py:69-80 upconv, :154-182 decoder BatchNorms, :199-260 the nine torch.cat, torchvision transitions),
-// sm_100a, HBM-bound.  All tensors are fp32 NHWC with an explicit pixel stride, so a channel slice of a wider slab is
+// sm_90a, HBM-bound.  All tensors are fp32 NHWC with an explicit pixel stride, so a channel slice of a wider slab is
 // read or written in place (concat = one vectorised slice copy per input instead of CatArrayBatchedCopy).
 //
 //   bts_bn_apply       out = x*scale + shift [ReLU]                    BatchNorm apply (train or folded eval stats)

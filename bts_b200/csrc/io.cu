@@ -1,4 +1,4 @@
-// The data formats on either side of the hot path (SURVEY 8f ranks 2 and 3), sm_100a, HBM-bound streaming kernels.
+// The data formats on either side of the hot path (SURVEY 8f ranks 2 and 3), sm_90a, HBM-bound streaming kernels.
 //
 //  bts_input_prep   the per-sample input transform of the reference loader, after decoding, fused with the H2D hand-off:
 //                   uint8 HWC frame (+ uint16 depth PNG) -> random crop -> horizontal flip -> gamma / brightness / colour

@@ -1,4 +1,4 @@
-// Local planar guidance (LPG) plane-to-depth up-sample, forward + backward, sm_100a.
+// Local planar guidance (LPG) plane-to-depth up-sample, forward + backward, sm_90a.
 //
 // Replaces: pytorch/bts.py:124-146 (local_planar_guidance.forward + its autograd backward, ~15-25
 // full-resolution ATen passes) and tensorflow/custom_layer/local_planar_guidance.cu:33-72 / 95-150.

@@ -1,5 +1,5 @@
 // Fused multi-tensor AdamW (decoupled weight decay) -- the optimizer step of the reference training loop
-// (pytorch/bts_main.py:371-373 torch.optim.AdamW over two parameter groups, :456-460 poly learning rate), sm_100a,
+// (pytorch/bts_main.py:371-373 torch.optim.AdamW over two parameter groups, :456-460 poly learning rate), sm_90a,
 // HBM-bound: every parameter of the model in ONE launch instead of torch's ~10 foreach kernels per group.
 //
 // Per element, in the operation order of torch's own multi-tensor implementation (torch/optim/adam.py _multi_tensor_adam)

@@ -1,11 +1,11 @@
 // Weight gradient of the narrow 1x1 convolutions of the reduction heads (reference pytorch/bts.py:83-108:
 // reduc1x1 32->16->8 at full resolution, reduc2x2 64->32->16->8->3 at half resolution, ...) as an HBM-bound CUDA-core
-// kernel, sm_100a.
+// kernel, sm_90a.
 //
 //   dW[co, ci] = sum_p dY[p, co] * x[p, ci]            Cin in {8,16,32,64}, Cout <= 32, NHWC operands
 //
-// On the tensor-core wgrad these layers fill 32 (or 8) of the 128 TMEM lanes and 16 (or 3) of the columns and still
-// pay the full operand-staging pipeline: round-1 trace 1.65 ms for 16->8 at 352x704x16 against 0.06 ms of HBM time.
+// On the tensor-core wgrad these layers fill 32 (or 8) of the 128 rows and 16 (or 3) of the columns of a tile and still
+// pay the full operand-staging pipeline, while the layer itself is HBM-bound.
 // Here a lane owns one (or two) input channels of one pixel slot and keeps all Cout accumulators in registers:
 // the x row of a pixel is one coalesced load, the dY row a broadcast load; pixel slots of a warp, warps of a block and
 // blocks are combined in a fixed order (shuffles, shared memory, a second pass over per-block partials) -> deterministic.
@@ -149,9 +149,8 @@ extern "C" int bts_conv_pw_wgrad(const float *x, long long x_pixel_stride, const
 }
 
 // ------------------------------------------------------------------------------------------------------------------
-// Forward / dgrad of the same narrow 1x1 layers (round 2).  On the tensor engine they ran at 2-16 TF/s -- 0.54 ms for
-// 32->16 at 352x704x16 against 0.12 ms of HBM time (profiles/r02_step_trace_*.txt): a 128x16 output tile leaves the MMA
-// at its 45-cycle floor while the full operand-staging pipeline still runs.  Here:
+// Forward / dgrad of the same narrow 1x1 layers.  These are HBM-bound (e.g. 32->16 at 352x704x16): on the tensor engine a
+// 128x16 output tile leaves the MMA nearly idle while the full operand-staging pipeline still runs.  Here:
 //   out[p, co] = act( sum_ci x[p, ci] * W[co, ci] )        dgrad: the same with W read transposed (x := dY)
 // A thread owns one pixel and one group of 4 output channels (the groups of a pixel are adjacent lanes, so the x row of a
 // pixel is a broadcast load and a warp writes 512 contiguous bytes); x sits in registers, the (transposed, zero-padded)

@@ -1,4 +1,4 @@
-// Scale-invariant log loss (silog_loss, pytorch/bts.py:41-48) forward + backward, sm_100a.
+// Scale-invariant log loss (silog_loss, pytorch/bts.py:41-48) forward + backward, sm_90a.
 //
 // The reference compacts est/gt with a boolean-mask index (nonzero + gather, twice), then runs ~8 small
 // ATen kernels; backward scatters back.  Here: ONE streaming pass reduces (sum d, sum d^2, N) over the

@@ -1,6 +1,7 @@
-// tcgen05 / TMEM / mbarrier / bulk-copy PTX wrappers shared by the tensor-core kernels (sm_100a).
+// wgmma / mbarrier / bulk-copy / TMA PTX wrappers shared by the tensor-core kernels (sm_90a).
 #pragma once
 #include "common.cuh"
+#include "wgmma_tf32.cuh"
 
 namespace tc {
 
@@ -30,9 +31,8 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (++spins > 200000000u) __trap();   // watchdog: a protocol bug must fail loudly, not hang the box
     }
 }
-// same protocol, for waits that are expected to be long (an epilogue warp waiting for a whole tile of MMAs, the
-// weight loader waiting for a free stage): back off between polls so the spinning lanes do not take issue slots
-// from the producer warps (ncu round 1: 30 % of all issued instructions were try_wait / branch / yield).
+// same protocol, for waits that are expected to be long (the weight loader waiting for a free stage): back off between
+// polls so the spinning lane does not take issue slots from the producer warps.
 __device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
     uint32_t ok = 0;
     uint32_t spins = 0;
@@ -54,7 +54,7 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void *src, uin
                  "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
-// TMA im2col load (cp.async.bulk.tensor ... .im2col -> SASS UTMALDG): `pixelsPerColumn` consecutive base pixels starting at
+// TMA im2col load (cp.async.bulk.tensor ... .im2col): `pixelsPerColumn` consecutive base pixels starting at
 // tensor coordinate (w, h, n), each shifted by the filter offset (off_w, off_h), `channelsPerPixel` channels from c; pixels
 // that fall outside the tensor (the convolution's zero padding) arrive as zeros.  Completes `bytes` on the mbarrier.
 __device__ __forceinline__ void tma_im2col_4d(uint32_t dst, const void *tmap, int c, int w, int h, int n, uint32_t bar,
@@ -76,65 +76,29 @@ __device__ __forceinline__ void tma_prefetch_desc(const void *tmap) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst, uint32_t ncols) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "r"(ncols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- warpgroup MMA (wgmma): ordering of the accumulator registers and of the asynchronous operand reads
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int PENDING>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(PENDING) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across an in-flight wgmma
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(tmem_d),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-}
-// one lane of a converged warp (elect.sync): the lane that issues the single-thread tcgen05 instructions
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xffffffff;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred));
-    return pred != 0;
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-                 : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-                 : "r"(taddr));
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, 128-byte swizzle shared-memory matrix descriptor (cute::UMMA::SmemDescriptor): start>>4 | LBO=1 |
-// SBO = 1024 B (8 rows x 128 B) | version 1 (sm_100) | layout SWIZZLE_128B (=2)
+// K-major, 128-byte swizzle shared-memory matrix descriptor (sm_90 wgmma): start>>4 | LBO (unused, 1) | SBO = 1024 B
+// (8 rows x 128 B) | layout SWIZZLE_128B (=1 at bits [62,64)).  Tiles are 1024-byte aligned; one k8 step of tf32 = +32 B.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 62);
 }
-// MN-major TF32 operands: the only layout the hardware accepts is SWIZZLE_128B_BASE32B (layout type 1,
-// cute Swizzle<2,5,2>): rows of 128 B (32 fp32 along MN), atoms of 4 K-rows (512 B), the 32-byte chunk index
-// (address bits [5,7)) XOR-ed with the K-row index mod 4 (address bits [7,9)).
-// The tile is [MN chunk of 32 fp32][K rows][128 B]; LBO = byte stride between MN chunks, SBO = 512 (4 K rows).
-__device__ __forceinline__ uint64_t make_desc_mn(uint32_t saddr, uint32_t lbo_bytes) {
-    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo_bytes >> 4) & 0x3FFFu) << 16) |
-           ((uint64_t)(512 >> 4) << 32) | (1ull << 46) | (1ull << 61);
-}
-// byte offset of 16-byte unit `unit` (0..7) of K-row `row` inside one MN chunk under that swizzle
-__device__ __forceinline__ uint32_t mn_swizzle_off(int row, int unit) {
-    return (uint32_t)row * 128u + (uint32_t)(((((unit >> 1) ^ (row & 3)) << 1) | (unit & 1)) << 4);
-}
-// instruction descriptor: D=f32, A=B=tf32, both K-major, N>>3 at [17,23), M>>4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int M, int N, int a_mn_major = 0, int b_mn_major = 0) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)a_mn_major << 15) | ((uint32_t)b_mn_major << 16) |
-           ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// K-major, no swizzle ("interleaved" core matrices of 8 rows x 16 B stored as 128 contiguous bytes): LBO = byte stride
+// between core matrices adjacent along K, SBO = byte stride between core matrices adjacent along M / N.
+__device__ __forceinline__ uint64_t make_desc_core(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+    return (uint64_t)((saddr >> 4) & 0x3FFFu) | ((uint64_t)((lbo >> 4) & 0x3FFFu) << 16) |
+           ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32);
 }
 
 __device__ __forceinline__ float rna_tf32(float x) {
@@ -194,6 +158,9 @@ __device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
     return v;
 }
 
+__device__ __forceinline__ void st_shared_f32(uint32_t addr, float a) {
+    asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory");
+}
 __device__ __forceinline__ void st_shared_v4(uint32_t addr, float a, float b, float c, float d) {
     asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }

@@ -1,4 +1,4 @@
-// Single-output-channel convolutions (Cout = 1) as HBM-bound CUDA-core kernels, sm_100a.
+// Single-output-channel convolutions (Cout = 1) as HBM-bound CUDA-core kernels, sm_90a.
 //
 // Replaces, for the two 1-channel heads of the BTS decoder -- `get_depth` (3x3, 32->1, + Sigmoid; reference
 // pytorch/bts.py:193-194,262) and `reduc1x1.reduc.final` (1x1, 8->1, + Sigmoid; bts.py:94-96) -- the cuDNN conv /

@@ -24,19 +24,19 @@ int bts_num_sms() {
     }
     if (!cached[dev]) {
         int n = 0;
-        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 148;   // B200
+        if (cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) n = 132;   // H100 SXM
         cached[dev] = n;
     }
     return (limit > 0 && limit < cached[dev]) ? limit : cached[dev];
 }
 
 extern "C" int bts_version(char *buf, int buflen) {
-    static const char v[] = "bts_b200 0.1 (sm_100a; lpg, plane_head, silog, conv_tc)";
+    static const char v[] = "bts_b200 0.1 (sm_90a; lpg, plane_head, silog, conv_tc)";
     if (buf && buflen > 0) {
         std::strncpy(buf, v, (size_t)buflen - 1);
         buf[buflen - 1] = 0;
     }
-    return 100;
+    return 90;
 }
 
 // zero n floats on the stream (grad_focal of the TF-op surface: `focal` never enters the LPG arithmetic, SURVEY Q1)

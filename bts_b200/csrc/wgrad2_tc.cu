@@ -1,24 +1,26 @@
 // wgrad for narrow-output 3x3 convolutions (Cout <= 64: the DenseNet 3x3 dense-layer convs 192->48 and the full- /
-// half-resolution decoder convs conv1/upconv1/conv2/upconv2) on tcgen05 + TMEM, 3xTF32 -- "shifted dY" formulation.
+// half-resolution decoder convs conv1/upconv1/conv2/upconv2) and for 1x1 layers with 64 < Cout <= 256, on the Hopper
+// tensor cores (wgmma, register accumulators), 3xTF32 -- "shifted dY" formulation.
 //
 //   dW[co, ci, tap] = sum_q  x~[q, ci] * dY[q - off(tap), co]            q = INPUT pixel, off(tap) = tap*dil - pad
 //
-// wgrad_tc.cu puts the tap in the grid, so the 128-channel activation tile -- the expensive operand: loads, BN/ReLU
-// pre-op, hi/lo split, 32 KB of shared-memory writes per k-block -- is produced 9 times, and with a narrow N the MMA
-// is too short to hide it (dense 3x3: 38 TF/s, conv1: 12 TF/s).  Here ONE CTA owns all taps of a (128 ci, <=48 co)
-// block: per k-block of 16 input pixels the activation tile is produced once and multiplied against the 9 shifted dY
-// tiles (cheap: <= 48 channels each), accumulating into 9 column blocks of TMEM (9 x 48 = 432 of 512 columns).
-// Same MN-major SWIZZLE_128B_BASE32B operand tiles and deterministic split-K partial layout as wgrad_tc.cu.
+// wgrad_tc.cu puts the tap in the grid, so the activation tile -- the expensive operand: loads, BN/ReLU pre-op, hi/lo
+// split, shared-memory writes per k-block -- is produced once per tap.  Here ONE CTA owns all taps of a (64 ci, cg co)
+// block: per k-block of 16 input pixels the activation tile is produced once and multiplied against the shifted dY tiles
+// of every tap, packed densely along N (tap t owns the N slots [t*ncol, (t+1)*ncol)), so that wgmma of width
+// taps*ncol <= 144 covers them all; two consumer warpgroups split those columns (<= 40 accumulator registers per thread).
+// Operand tiles are K-major (pixels contiguous per channel row) in 8 x 16-byte core matrices, written by the producers;
+// deterministic split-K partial layout as wgrad_tc.cu.
 //
-// Operand staging (round 2): the 9 shifted dY windows of a k-block overlap -- they are KH row segments of 16 + (KW-1)*dil
-// consecutive output pixels -- and ncu showed the producers 58% stalled on the scoreboard of their global loads (one k-block
-// of register prefetch, L1 hit rate 13%).  With TMA = true a loader lane copies the raw fp32 segments (and the raw x tile
-// unless it is read through the nearest-neighbour up-sample) into a small landing ring, several k-blocks ahead
-// (cp.async.bulk.tensor.2d, no swizzle, zero fill past the tensor ends); the producers then read shared memory, apply the
-// border masks / pre-op, split hi/lo and write the swizzled operand tiles as before.
+// Operand staging: the shifted dY windows of a k-block overlap -- they are KH row segments of 16 + (KW-1)*dil consecutive
+// output pixels.  With TMA = true a loader lane copies the raw fp32 segments (and the raw x tile unless it is read through
+// the nearest-neighbour up-sample) into a small landing ring, several k-blocks ahead (cp.async.bulk.tensor.2d, no swizzle,
+// zero fill past the tensor ends); the producers then read shared memory, apply the border masks / pre-op, split hi/lo
+// and write the operand tiles.
 #include <cuda.h>
 
 #include <cstring>
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -26,17 +28,22 @@ using namespace tc;
 
 namespace {
 
-constexpr int BLOCK_CI = 128;
+constexpr int BLOCK_CI = 64;                 // input channels per CTA = the M of one consumer warpgroup
+constexpr int X_CHUNKS = BLOCK_CI / 32;      // 32-channel chunks of the activation tile
 constexpr int KP = 16;                       // input pixels per k-block (2 k-groups of 8)
-constexpr int CHUNK = KP * 128;              // one 32-channel chunk of a k-block: 2 KB
-constexpr int A_BYTES = 4 * CHUNK;           // 8 KB (hi or lo)
+constexpr uint32_t CORE_SBO = 4 * 128 + 16;  // one 8-row group of a k-block: 4 core matrices along K + a bank pad
+constexpr int A_BYTES = BLOCK_CI / 8 * CORE_SBO;   // hi or lo
 constexpr int MAX_TAPS = 9;
+constexpr int MAX_NT = 144;                  // widest packed N (taps * ncol), split between the two consumer warpgroups
 constexpr int MAX_STAGES = 4;
-constexpr int NUM_THREADS = 576;               // 2 control warps + 16 producer warps (4 quarters of 128 threads)
-constexpr int PRODUCERS = 512;
+constexpr int CONSUMER_THREADS = 256;       // two warpgroups, each owns about half of the packed N columns
+constexpr int LOADER_WARP = CONSUMER_THREADS / 32;
+constexpr int GROUPS = 3;                    // producer groups of 128 threads: group g owns the dY taps t == g (mod 3)
+constexpr int PRODUCERS = 128 * GROUPS;
+constexpr int NUM_THREADS = CONSUMER_THREADS + 32 + PRODUCERS;
 constexpr int SMEM_BUDGET = 224 * 1024;
 constexpr int MAX_RING = 4;                  // landing-ring slots (TMA staging)
-constexpr int X_RAW_BYTES = KP * BLOCK_CI * 4;   // raw x tile of a k-block: 8 KB
+constexpr int X_RAW_BYTES = KP * BLOCK_CI * 4;   // raw x tile of a k-block: 4 KB
 
 struct W2Params {
     const float *x; long long xs;
@@ -45,14 +52,13 @@ struct W2Params {
     const float *pre_scale, *pre_shift;
     const float *dy; long long dys;
     int Cout, Hout, Wout, Hin, Win;
-    int cg, nb;              // output channels per CTA (multiple of 16, <= 48) and their 32-channel chunks
-    int nchunks;             // 32-slot chunks of the tap-packed dY tile: ceil(taps*cg/32)
+    int cg, nb;              // output channels per CTA (multiple of 16) and their 32-channel chunks
+    int nchunks;             // 32-row chunks of the tap-packed dY tile: ceil(taps*cg/32)
     float *part;             // [splitK][taps][Cin][Cout]
     int splitK, kb_per_split, KBq;
     int Mq;                  // B*Hin*Win input pixels
     int stages, stage_bytes, precision;
-    int legacy;              // 1: round-1 single-lane MMA issue loop (fallback switch)
-    // TMA landing ring (TMA = true): slot = [raw x tile 8 KB (unless up) | KH segments of segw pixels x cg channels]
+    // TMA landing ring (TMA = true): slot = [raw x tile (unless up) | KH segments of segw pixels x cg channels]
     int ring, slot_bytes, seg_bytes, segw, tox_max, slot_tx;
 };
 
@@ -69,24 +75,20 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + BLOCK_CI;
     const uint32_t bar0 = base + pre_off + 2 * BLOCK_CI * 4;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + pre_off + 2 * BLOCK_CI * 4);
     auto full = [&](int s) { return bar0 + 8u * s; };
     auto empty = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
-    const uint32_t accum_full = bar0 + 8u * (2 * MAX_STAGES);
-    auto rfull = [&](int j) { return bar0 + 8u * (2 * MAX_STAGES + 1 + j); };
-    auto rempty = [&](int j) { return bar0 + 8u * (2 * MAX_STAGES + 1 + MAX_RING + j); };
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * MAX_STAGES + 1 + 2 * MAX_RING);
-
+    auto rfull = [&](int j) { return bar0 + 8u * (2 * MAX_STAGES + j); };
+    auto rempty = [&](int j) { return bar0 + 8u * (2 * MAX_STAGES + MAX_RING + j); };
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int ci_tile = blockIdx.x, cgi = blockIdx.y, split = blockIdx.z;
     const int co0 = cgi * p.cg;
     const int ncol = min(p.cg, ((p.Cout - co0 + 15) >> 4) << 4);     // live columns of this CTA (multiple of 16)
     const int nb = p.nb;
-    // dY operand: the taps are packed DENSELY along N -- tap t owns the N slots [t*ncol, (t+1)*ncol) of one long MN-major
-    // tile of ceil(taps*ncol/32) chunks -- so that a single tcgen05.mma (N up to 256) multiplies the activation tile
-    // against many taps at once (see the MMA issuer).  hi and lo tiles follow each other.
+    // dY operand: the taps are packed DENSELY along N -- tap t owns the N rows [t*ncol, (t+1)*ncol) of one tile of
+    // ceil(taps*ncol/32) 32-row chunks -- so that a single wgmma multiplies the activation tile against all taps at once.
+    // hi and lo tiles follow each other.
     const int n_total = taps * ncol;
-    const uint32_t b_half = (uint32_t)p.nchunks * CHUNK;
+    const uint32_t b_half = (uint32_t)p.nchunks * 4u * CORE_SBO;
     const int kb0 = split * p.kb_per_split;
     int kb1 = kb0 + p.kb_per_split;
     if (kb1 > p.KBq) kb1 = p.KBq;
@@ -95,16 +97,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
     if (threadIdx.x == 0) {
         for (int s = 0; s < MAX_STAGES; ++s) {
             mbar_init(full(s), PRODUCERS);
-            mbar_init(empty(s), 1);
+            mbar_init(empty(s), CONSUMER_THREADS);
         }
-        mbar_init(accum_full, 1);
         for (int j = 0; j < MAX_RING; ++j) {
             mbar_init(rfull(j), 1);
             mbar_init(rempty(j), PRODUCERS);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 512);
     if (PRE >= 2) {
         for (int c = threadIdx.x; c < BLOCK_CI; c += NUM_THREADS) {
             const int ch = ci_tile * BLOCK_CI + c;
@@ -115,14 +115,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
     // zero every operand stage once: dead channel chunks / dead units are never written afterwards
     for (int i = threadIdx.x; i < S * p.stage_bytes / 16; i += NUM_THREADS) st_shared_v4(base + i * 16, 0.f, 0.f, 0.f, 0.f);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (TMA && warp == 0) {
+    if (warp == LOADER_WARP) {
         // ---- loader: one lane keeps the landing ring `ring` k-blocks ahead of the producers
-        if (lane == 0) {
+        if (TMA && lane == 0) {
             if (!UP) tma_prefetch_desc(&tmx);
             tma_prefetch_desc(&tmd);
             int j = 0;
@@ -143,105 +140,95 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 if (++j == p.ring) { j = 0; ph ^= 1; }
             }
         }
-    } else if (warp == 1) {
-        // MMA issuer: whole warp in the loop, one elected lane issues (see conv_tc.cu: the round-1 single-lane loops paid
-        // ~4 cycles x hundreds of issue-warp instructions per k-block).  With the taps packed along N the three products
-        // of a k-group are 3 x ceil(taps*ncol/256) instructions instead of 3 x taps.
-        if (p.legacy) {
-        if (lane == 0) {
-            // A tcgen05.mma with M=128, K=8 costs ~115-130 cycles whatever N is (round-1 measurement: 54 per-tap MMAs
-            // per 16-pixel k-block = 5.5k cycles, exactly the observed k-block time).  With the taps packed along N the
-            // three products of a k-group are 3 x ceil(taps*ncol/256) instructions instead of 3 x taps.
-            const int n0 = n_total < 256 ? n_total : 256, n1 = n_total - n0;        // multiples of 16
-            const uint32_t idesc0 = make_idesc(BLOCK_CI, n0, 1, 1);
-            const uint32_t idesc1 = make_idesc(BLOCK_CI, n1 > 0 ? n1 : 16, 1, 1);
-            const uint64_t dah0 = make_desc_mn(base, CHUNK), dal0 = make_desc_mn(base + A_BYTES, CHUNK);
-            const uint64_t dbh0 = make_desc_mn(base + 2 * A_BYTES, CHUNK), dbl0 = make_desc_mn(base + 2 * A_BYTES + b_half, CHUNK);
-            const uint64_t piece1 = (uint64_t)((8 * CHUNK) >> 4), stage_step = (uint64_t)(p.stage_bytes >> 4);
+    } else if (warp < LOADER_WARP) {
+        // ---- consumer warpgroups: rows = the 64 input channels; warpgroup wg owns the packed columns [n0, n0 + N) of
+        //      all taps x ncol (n0 = 0 | the first half rounded up to 16); 3xTF32 per k8 step, small cross terms first;
+        //      a stage is released as soon as its wgmma group has completed
+        const int wg = warp >> 2;
+        const int n_half = (n_total + 31) / 32 * 16;
+        const int n0 = wg ? n_half : 0, n_mine = wg ? n_total - n_half : n_half;
+        auto consume = [&](auto NT) {
+            constexpr int N = decltype(NT)::value;
+            float acc[N > 0 ? N / 2 : 1];
+#pragma unroll
+            for (int i = 0; i < (N > 0 ? N / 2 : 1); ++i) acc[i] = 0.f;
+            const bool single = p.precision != 0;
             int s = 0;
             uint32_t ph = 0;
             for (int it = 0; it < nkb; ++it) {
                 mbar_wait(full(s), ph);
-                tc_fence_after();
-                const uint64_t so = (uint64_t)s * stage_step;
+                wgmma_fence();
+                const uint32_t a_hi = base + (uint32_t)s * (uint32_t)p.stage_bytes, a_lo = a_hi + A_BYTES;
+                const uint32_t b_hi = a_hi + 2 * A_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO, b_lo = b_hi + b_half;
+                if constexpr (N > 0) {
 #pragma unroll
-                for (int kg = 0; kg < KP / 8; ++kg) {
-                    const uint64_t o = so + (uint64_t)(kg * (1024 >> 4));   // start-address field: + 1024 B per k-group
-                    const uint32_t accumulate = (it | kg) != 0;
-                    if (p.precision == 0) {
-                        umma_tf32(tmem_base, dal0 + o, dbh0 + o, idesc0, accumulate);
-                        umma_tf32(tmem_base, dah0 + o, dbl0 + o, idesc0, 1);
-                        umma_tf32(tmem_base, dah0 + o, dbh0 + o, idesc0, 1);
-                        if (n1 > 0) {
-                            umma_tf32(tmem_base + 256, dal0 + o, dbh0 + o + piece1, idesc1, accumulate);
-                            umma_tf32(tmem_base + 256, dah0 + o, dbl0 + o + piece1, idesc1, 1);
-                            umma_tf32(tmem_base + 256, dah0 + o, dbh0 + o + piece1, idesc1, 1);
+                    for (int kg = 0; kg < KP / 8; ++kg) {
+                        const uint32_t ko = (uint32_t)kg * 256u;
+                        const uint64_t dah = make_desc_core(a_hi + ko, 128, CORE_SBO), dal = make_desc_core(a_lo + ko, 128, CORE_SBO);
+                        const uint64_t dbh = make_desc_core(b_hi + ko, 128, CORE_SBO), dbl = make_desc_core(b_lo + ko, 128, CORE_SBO);
+                        const uint32_t accumulate = (it | kg) != 0;
+                        if (single) {
+                            Wgmma<N>::mma(acc, dah, dbh, accumulate);
+                        } else {
+                            Wgmma<N>::mma(acc, dal, dbh, accumulate);
+                            Wgmma<N>::mma(acc, dah, dbl, 1);
+                            Wgmma<N>::mma(acc, dah, dbh, 1);
                         }
-                    } else {
-                        umma_tf32(tmem_base, dah0 + o, dbh0 + o, idesc0, accumulate);
-                        if (n1 > 0) umma_tf32(tmem_base + 256, dah0 + o, dbh0 + o + piece1, idesc1, accumulate);
                     }
                 }
-                umma_commit(empty(s));
+                wgmma_commit();
+                wgmma_wait<0>();
+                mbar_arrive(empty(s));
                 if (++s == S) { s = 0; ph ^= 1; }
             }
-            umma_commit(accum_full);
-        }
-        } else {
-        const int n0 = n_total < 256 ? n_total : 256, n1 = n_total - n0;        // multiples of 16
-        const uint32_t idesc0 = make_idesc(BLOCK_CI, n0, 1, 1);
-        const uint32_t idesc1 = make_idesc(BLOCK_CI, n1 > 0 ? n1 : 16, 1, 1);
-        const uint64_t dah0 = make_desc_mn(base, CHUNK), dal0 = make_desc_mn(base + A_BYTES, CHUNK);
-        const uint64_t dbh0 = make_desc_mn(base + 2 * A_BYTES, CHUNK), dbl0 = make_desc_mn(base + 2 * A_BYTES + b_half, CHUNK);
-        const uint64_t piece1 = (uint64_t)((8 * CHUNK) >> 4), stage_step = (uint64_t)(p.stage_bytes >> 4);
-        const bool leader = elect_one();
-        const bool two = n1 > 0, single = p.precision != 0;
-        int s = 0;
-        uint32_t ph = 0;
-        uint64_t so = 0;
-        uint32_t bfull = full(0), bempty = empty(0);
-        for (int it = 0; it < nkb; ++it) {
-            mbar_wait(bfull, ph);
-            tc_fence_after();
-            if (leader) {
+            wgmma_wait<0>();
+            wgmma_fence_operands(acc);
+            if (N == 0) return;
+            // ---- epilogue: accumulator row = input channel, column n = tap (n / ncol), output channel co0 + n % ncol
+            const bool ovec = (p.Cout & 1) == 0 && ((((uintptr_t)p.part) & 7) == 0) && ((co0 & 1) == 0);
 #pragma unroll
-                for (int kg = 0; kg < KP / 8; ++kg) {
-                    const uint64_t o = so + (uint64_t)(kg * (1024 >> 4));   // start-address field: + 1024 B per k-group
-                    const uint32_t accumulate = kg != 0 ? 1u : (uint32_t)(it != 0);
-                    if (!single) {
-                        umma_tf32(tmem_base, dal0 + o, dbh0 + o, idesc0, accumulate);
-                        umma_tf32(tmem_base, dah0 + o, dbl0 + o, idesc0, 1);
-                        umma_tf32(tmem_base, dah0 + o, dbh0 + o, idesc0, 1);
-                        if (two) {
-                            umma_tf32(tmem_base + 256, dal0 + o, dbh0 + o + piece1, idesc1, accumulate);
-                            umma_tf32(tmem_base + 256, dah0 + o, dbl0 + o + piece1, idesc1, 1);
-                            umma_tf32(tmem_base + 256, dah0 + o, dbh0 + o + piece1, idesc1, 1);
-                        }
+            for (int i = 0; i < 2; ++i) {
+                const int ci = ci_tile * BLOCK_CI + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+                if (ci >= p.Cin) continue;
+#pragma unroll
+                for (int j = 0; j < (N > 0 ? N / 8 : 0); ++j) {
+                    const int n = n0 + 8 * j + (lane & 3) * 2;
+                    if (n >= n0 + n_mine) continue;
+                    const int t = n / ncol, cc = n - t * ncol;
+                    float *dst = p.part + (((long long)split * taps + t) * p.Cin + ci) * p.Cout + co0 + cc;
+                    const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+                    if (ovec && co0 + cc + 1 < p.Cout) {
+                        *reinterpret_cast<float2 *>(dst) = make_float2(v0, v1);
                     } else {
-                        umma_tf32(tmem_base, dah0 + o, dbh0 + o, idesc0, accumulate);
-                        if (two) umma_tf32(tmem_base + 256, dah0 + o, dbh0 + o + piece1, idesc1, accumulate);
+                        if (co0 + cc < p.Cout) dst[0] = v0;
+                        if (co0 + cc + 1 < p.Cout) dst[1] = v1;
                     }
                 }
-                umma_commit(bempty);
-                if (it == nkb - 1) umma_commit(accum_full);
             }
-            __syncwarp();
-            so += stage_step; bfull += 8u; bempty += 8u;
-            if (++s == S) { s = 0; ph ^= 1; so = 0; bfull = full(0); bempty = empty(0); }
+        };
+        switch (n_mine) {
+            case 0: consume(std::integral_constant<int, 0>()); break;       // nothing to multiply: only releases stages
+            case 16: consume(std::integral_constant<int, 16>()); break;
+            case 32: consume(std::integral_constant<int, 32>()); break;
+            case 48: consume(std::integral_constant<int, 48>()); break;
+            case 64: consume(std::integral_constant<int, 64>()); break;
+            default: consume(std::integral_constant<int, 80>()); break;
         }
-        if (nkb == 0 && leader) umma_commit(accum_full);
-        }   // lean issue loop
-    } else if (warp >= 2) {
-        // 16 producer warps (round 1 ran 8: ncu showed ~9 cycles between a warp's instructions and 2.5 warps per
-        // scheduler -- the per-thread instruction stream, not the tensor pipe, set the k-block time).  Quarter q of the
-        // producers owns the x chunk q and the dY taps t == q (mod 4): at most 1 + 6 sixteen-byte units per thread.
-        const int pt = threadIdx.x - 64;           // 0..511
+    } else {
+        // 12 producer warps in GROUPS = 3 groups of 128 threads.  Group q owns the x chunk q (if any) and the dY taps
+        // t == q (mod 3): at most 1 + 6 sixteen-byte units per thread.
+        const int pt = threadIdx.x - (CONSUMER_THREADS + 32);   // 0..PRODUCERS-1
         const int unit = pt & 7;                   // 16-byte unit of the 128-byte row
         const int row = (pt >> 3) & 15;            // pixel row of the 16-pixel k-block
-        const int half = pt >> 7;                  // quarter 0..3: A chunk `half`;  dY: taps t == half (mod 4)
+        const int half = pt >> 7;                  // group 0..2: A chunk `half` (< X_CHUNKS);  dY: taps t == half (mod 3)
+        const bool xq = half < X_CHUNKS;
         constexpr bool AFF = PRE >= 2;
         constexpr bool RELU = (PRE & 1) != 0;
-        const uint32_t roff = mn_swizzle_off(row, unit);
+        // K-major core-matrix tiles: element (row n, pixel k) at (n / 8) * CORE_SBO + (k / 4) * 128 + (n % 8) * 16 + (k % 4) * 4;
+        // a thread's 4 consecutive channels of one pixel are 4 scalar stores 16 bytes apart
+        auto core_off = [&](int n) {
+            return (uint32_t)(n >> 3) * CORE_SBO + (uint32_t)(row >> 2) * 128u + (uint32_t)(n & 7) * 16u + (uint32_t)(row & 3) * 4u;
+        };
         const int xs = (int)p.xs, dys = (int)p.dys;
         const int cbx = ci_tile * BLOCK_CI + half * 32 + unit * 4;    // first x channel of this thread (chunk `half`)
         const int cbd = co0 + unit * 4;                               // first dY channel (chunk 0)
@@ -251,8 +238,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
         if (AFF) {
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
-                sc[0][e] = s_scale[half * 32 + unit * 4 + e];
-                sh[0][e] = s_shift[half * 32 + unit * 4 + e];
+                sc[0][e] = xq ? s_scale[half * 32 + unit * 4 + e] : 0.f;
+                sh[0][e] = xq ? s_shift[half * 32 + unit * 4 + e] : 0.f;
             }
         }
         // input-pixel coordinates of this thread's row, advanced by 16 pixels per k-block (no divisions in the loop)
@@ -266,11 +253,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
         }
         constexpr int NBU = 6;                     // dY units per thread per k-block: <= 3 taps x 2 chunks
         constexpr int NAU = 1;                     // x units per thread per k-block
-        // Unit slots (j, ch), j = 0..2, ch = 0..1.  Multi-tap layers: tap t = half + 4j, 32-channel chunk ch of <= 2.
-        // Single-tap (1x1) layers: tap 0, chunk half + 4*(2j + ch) of <= 8 (an output tile up to 256 channels wide).
+        // Unit slots (j, ch), j = 0..2, ch = 0..1.  Multi-tap layers: tap t = half + 3j, 32-channel chunk ch of <= 2.
+        // Single-tap (1x1) layers: tap 0, chunk half + 3*(2j + ch) of <= 4 (an output tile up to 128 channels wide).
         const bool single = taps == 1;
-        auto unit_tap = [&](int j) { return single ? 0 : half + 4 * j; };
-        auto unit_chunk = [&](int j, int ch) { return single ? half + 4 * (2 * j + ch) : ch; };
+        auto unit_tap = [&](int j) { return single ? 0 : half + GROUPS * j; };
+        auto unit_chunk = [&](int j, int ch) { return single ? half + GROUPS * (2 * j + ch) : ch; };
         // tap offsets of this thread's taps, computed once: no divisions in the k-loop
         int toy[NBU / 2], tox[NBU / 2], tky[NBU / 2];
 #pragma unroll
@@ -292,7 +279,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 const int c = unit * 4 + cc * 32;                         // channel within this CTA's group
                 const int n = t * ncol + c;
                 blive[j * 2 + ch] = t < taps && cc < nb && c < ncol;
-                boff[j * 2 + ch] = (uint32_t)(n >> 5) * CHUNK + mn_swizzle_off(row, (n & 31) >> 2);
+                boff[j * 2 + ch] = core_off(n);
             }
         struct Cursor { int qx, qy, qb; };
         Cursor cur = {qx, qy, qb};
@@ -312,7 +299,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
 #pragma unroll
             for (int ch = 0; ch < NAU; ++ch) {
                 const int c = cbx + ch * 32;
-                const bool live = okx && c < p.Cin;
+                const bool live = xq && okx && c < p.Cin;
                 if (VEC) {
                     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
                     if (live) v = __ldg(reinterpret_cast<const float4 *>(xg + xoff + c));
@@ -376,7 +363,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
             okx = q < p.Mq;
             uint32_t segb = slot;
             if (!UP) {
-                const float4 v = ld_shared_v4(slot + (uint32_t)((row * BLOCK_CI + half * 32 + unit * 4) * 4));
+                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (xq) v = ld_shared_v4(slot + (uint32_t)((row * BLOCK_CI + half * 32 + unit * 4) * 4));
                 va[0].v[0] = v.x; va[0].v[1] = v.y; va[0].v[2] = v.z; va[0].v[3] = v.w;    // channels >= Cin, pixels >= Mq: zero fill
                 segb += X_RAW_BYTES;
             }
@@ -406,8 +394,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 hi[e] = hh;
                 lo[e] = a - hh;
             }
-            st_shared_v4(hi_addr, hi[0], hi[1], hi[2], hi[3]);
-            st_shared_v4(lo_addr, lo[0], lo[1], lo[2], lo[3]);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                st_shared_f32(hi_addr + 16u * e, hi[e]);
+                st_shared_f32(lo_addr + 16u * e, lo[e]);
+            }
         };
         int st_s = 0;
         uint32_t st_ph = 0;
@@ -434,10 +425,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
             mbar_wait(empty(s), ph ^ 1);
             const uint32_t a_hi = base + (uint32_t)s * (uint32_t)p.stage_bytes, a_lo = a_hi + A_BYTES;
             const uint32_t b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + b_half;
-#pragma unroll
-            for (int ch = 0; ch < NAU; ++ch) {
-                const uint32_t o = (uint32_t)(half + ch) * CHUNK + roff;
-                split_store(a_hi + o, a_lo + o, va[ch]);
+            if (xq) {
+                const uint32_t o = core_off(half * 32 + unit * 4);
+                split_store(a_hi + o, a_lo + o, va[0]);
             }
 #pragma unroll
             for (int j = 0; j < NBU; ++j)
@@ -483,52 +473,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 }
             }
         }
-
-        // ---- epilogue: TMEM lane = input channel; column block t*ncol.. = tap t; taps split between the two halves
-        mbar_wait(accum_full, 0);
-        tc_fence_after();
-        const int q4 = warp & 3;
-        const int ci = ci_tile * BLOCK_CI + q4 * 32 + lane;
-        const bool ovec = (p.Cout & 3) == 0 && ((((uintptr_t)p.part) & 15) == 0) && ((co0 & 3) == 0);
-        // multi-tap: the taps are split between the four quarters; single-tap: the 8-column blocks of the one tap are
-        for (int t = single ? 0 : half; t < taps; t += single ? 1 : 4) {
-            float *prow = p.part + (((long long)split * taps + t) * p.Cin + (ci < p.Cin ? ci : 0)) * p.Cout + co0;
-            for (int cc = single ? half * 8 : 0; cc < ncol; cc += single ? 32 : 8) {
-                uint32_t r[8];
-                tmem_ld8(tmem_base + ((uint32_t)(q4 * 32) << 16) + (uint32_t)(t * ncol + cc), r);
-                tmem_ld_wait();
-                if (ci < p.Cin) {
-#pragma unroll
-                    for (int e4 = 0; e4 < 8; e4 += 4) {
-                        const int c = co0 + cc + e4;
-                        if (ovec && c + 3 < p.Cout) {
-                            *reinterpret_cast<float4 *>(prow + cc + e4) =
-                                make_float4(nkb ? __uint_as_float(r[e4]) : 0.f, nkb ? __uint_as_float(r[e4 + 1]) : 0.f,
-                                            nkb ? __uint_as_float(r[e4 + 2]) : 0.f, nkb ? __uint_as_float(r[e4 + 3]) : 0.f);
-                        } else {
-#pragma unroll
-                            for (int e = 0; e < 4; ++e)
-                                if (c + e < p.Cout) prow[cc + e4 + e] = nkb ? __uint_as_float(r[e4 + e]) : 0.f;
-                        }
-                    }
-                }
-            }
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace
 
-int bts_issue_legacy();
-
-// co-group width for the shifted-dY kernel: multiple of 16, taps*cg <= 512 TMEM columns, groups as even as possible
+// co-group width for the shifted-dY kernel: multiple of 16, taps*cg <= MAX_NT accumulator columns, groups as even as possible
 int bts_wgrad2_cg(int Cout, int taps) {
-    int cap = (512 / taps) / 16 * 16;
+    int cap = (MAX_NT / taps) / 16 * 16;
     if (taps == 1) {
-        if (cap > 256) cap = 256;              // 1x1: one tile up to 256 output channels wide (one tcgen05.mma)
+        if (cap > 128) cap = 128;              // 1x1: output tiles up to 128 channels wide
     } else if (cap > 48) {
         cap = 48;
     }
@@ -539,9 +493,8 @@ int bts_wgrad2_cg(int Cout, int taps) {
     return cg;
 }
 
-// measured (B200, K16 shapes, profiles/r02_w2_sweep.txt): with the TMA landing ring it beats the tap-in-grid kernel on
-// every narrow-output 3x3 layer down to the 22x44 maps of block 3 (40 vs 71 us with >= 8 k-blocks per split-K CTA and one
-// wave of CTAs); on the 11x22 maps of block 4 (3.9k pixels) the two tie and the tap-in-grid kernel stays
+// used on maps of at least 12k pixels (down to the 22x44 maps of DenseNet block 3 at batch 16) with >= 8 k-blocks per
+// split-K CTA; smaller maps stay on the tap-in-grid kernel
 static long long g_w2_min_pixels = 12000;
 static int g_w2_pointwise = 1;               // 1x1 layers (64 < Cout <= 256) on this kernel too
 extern "C" int bts_wgrad2_set_pointwise(int on) { g_w2_pointwise = on ? 1 : 0; return 0; }
@@ -552,7 +505,7 @@ extern "C" int bts_wgrad2_set_min_kblocks(int n) { g_w2_min_kb = n < 1 ? 8 : n; 
 bool bts_wgrad2_eligible(int Cout, int KH, int KW, int stride, long long Mq) {
     const int taps = KH * KW;
     if (stride != 1 || Mq < g_w2_min_pixels || taps > MAX_TAPS || bts_wgrad2_cg(Cout, taps) <= 0) return false;
-    if (taps == 1) return g_w2_pointwise && Cout > 64 && Cout <= 256;   // 1x1 layers with one <= 256-wide output tile
+    if (taps == 1) return g_w2_pointwise && Cout > 64 && Cout <= 256;   // 1x1 layers with 64 < Cout <= 256
     return Cout <= 64;
 }
 
@@ -633,12 +586,11 @@ int bts_wgrad2_launch(const float *x, long long xs, int B, int Hs, int Ws, int u
     p.KBq = (int)((Mq + KP - 1) / KP);
     p.kb_per_split = (p.KBq + splitK - 1) / splitK;
     p.nchunks = (taps * p.cg + 31) / 32;
-    p.stage_bytes = 2 * A_BYTES + 2 * p.nchunks * CHUNK;
+    p.stage_bytes = 2 * A_BYTES + 2 * p.nchunks * 4 * (int)CORE_SBO;
     p.stages = SMEM_BUDGET / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     if (p.stages < 2) return BTS_EINVAL;
     p.precision = precision;
-    p.legacy = bts_issue_legacy();
     const int pre = (pre_scale ? 2 : 0) | (pre_relu ? 1 : 0);
     const bool vec = bts_aligned16(x) && (xs % 4 == 0) && bts_aligned16(dy) && (dys % 4 == 0);
     // ---- landing ring (TMA): 'same' convolutions with <= 3 kernel rows; 3 operand stages if >= 3 ring slots still fit, else 2

@@ -1,17 +1,16 @@
-// Weight-gradient (wgrad) of the implicit-GEMM convolution on tcgen05 + TMEM, sm_100a, 3xTF32.
+// Weight-gradient (wgrad) of the implicit-GEMM convolution on the Hopper tensor cores (wgmma), sm_90a, 3xTF32.
 //
 //   dW[co, ci, tap] = sum_p  dY[p, co] * pre(x[p (+) tap, ci])            (same pre / (+) as conv_tc.cu)
 //
-// GEMM view per (tap, split):  M = 128 input channels (TMEM lanes), N = n_tile output channels, K = output pixels.
-// Both operands live in memory as [pixel][channel] (NHWC), i.e. the reduction index is the slow one, so both shared
-// memory tiles are "MN-major": [32-channel chunk][32 pixel rows][128 B] in the SWIZZLE_128B_BASE32B pattern (the only
-// one the tensor core accepts for MN-major TF32), UMMA descriptors with a_major = b_major = MN, LBO = chunk stride.
-// grid = (ceil(Cin/128), n_tiles(Cout), taps * splitK); each CTA reduces its pixel range into an fp32 TMEM tile and
-// writes a partial; a second, deterministic kernel sums the splitK partials into the (Cout,Cin,KH,KW)-strided gradient.
-// n_tile <= 128: two tcgen05.mma per k-group (x_hi^T*[dY_hi;dY_lo] as one instruction of width 32*nchunk + n_tile, then
-// x_lo^T*dY_hi); 128 < n_tile <= 256: one tile, three plain products, the dY tile produced in two passes of 4 chunks.
-// 576 threads: MMA issuer warp + 2 producer groups of 8 warps (x tile / dY tile), 2-4 operand stages as smem allows.
+// GEMM view per (tap, split):  M = 128 input channels (two consumer warpgroups of 64), N = n_tile <= 64 output channels,
+// K = output pixels.  Both operands live in memory as [pixel][channel] (NHWC), i.e. the reduction index is the slow one,
+// while tf32 wgmma reads only K-major operands: the producers transpose on their way into shared memory, writing
+// [channel][pixel] tiles of 8 x 16-byte core matrices (no swizzle).
+// grid = (ceil(Cin/128), n_tiles(Cout), taps * splitK); each CTA reduces its pixel range into fp32 register accumulators
+// and writes a partial; a second, deterministic kernel sums the splitK partials into the (Cout,Cin,KH,KW)-strided gradient.
+// 768 threads: 2 consumer warpgroups + 2 producer groups of 8 warps (x tile / dY tile), 2-4 operand stages.
 #include <cstdlib>
+#include <type_traits>
 
 #include "tc_common.cuh"
 
@@ -21,13 +20,14 @@ namespace {
 
 constexpr int BLOCK_CI = 128;
 constexpr int BLOCK_KP = 32;                 // pixels per k-block
-constexpr int MAX_N = 256;                   // output channels per CTA tile (one tcgen05.mma covers up to 256)
+constexpr int MAX_N = 64;                    // output channels per CTA tile (register accumulator of the consumers)
 constexpr int MAX_STAGES = 4;
 constexpr int SMEM_LIMIT = 232448;
-constexpr int CHUNK_BYTES = BLOCK_KP * 128;  // one 32-channel chunk of a k-block: 4 KB
-constexpr int A_BYTES = 4 * CHUNK_BYTES;     // 16 KB (hi or lo)
-constexpr int NUM_THREADS = 576;               // 2 control warps + 2 producer groups x 8 warps
+constexpr uint32_t CORE_SBO = 8 * 128 + 16;  // one 8-channel group of a k-block: 8 core matrices along K + a bank pad
+constexpr int A_BYTES = 16 * CORE_SBO;       // 128 channels (hi or lo)
+constexpr int CONSUMER_THREADS = 256;
 constexpr int GROUP_THREADS = 256;
+constexpr int NUM_THREADS = CONSUMER_THREADS + 2 * GROUP_THREADS;
 
 struct WgradParams {
     const float *x; long long xs;
@@ -37,13 +37,13 @@ struct WgradParams {
     const float *dy; long long dys;
     int Cout, Hout, Wout;
     int n_tile;
-    int legacy;              // 1: round-1 single-lane MMA issue loop (fallback switch, bts_conv_set_issue_mode(0))
-    int kwin;                // grouped (block-diagonal) layer: only the tiles ci_tile == nt exist, n_tile == kwin == 128
+    int kwin;                // grouped (block-diagonal) layer: only the n-tiles inside the diagonal block ci_tile exist
     float *part;             // [splitK][taps][Cin][Cout]   (grouped: [splitK][taps][Cin][kwin])
     int splitK, kb_per_split, KBp;
     int M;
     int x_vec, dy_vec, precision;
-    int stages, stage_bytes;     // operand ring: [A hi 16K | A lo 16K | dY hi nchunk*4K | dY lo nchunk*4K] per stage
+    int stages, stage_bytes;     // operand ring: [A hi | A lo | dY hi b_bytes | dY lo b_bytes] per stage
+    int b_bytes;
 };
 
 
@@ -58,18 +58,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
     const uint32_t bar_off = pre_off + 2 * BLOCK_CI * 4;
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + BLOCK_CI;
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sm + bar_off);
     const uint32_t bar0 = base + bar_off;
     auto full = [&](int s) { return bar0 + 8u * s; };
     auto empty = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
-    const uint32_t accum_full = bar0 + 8u * (2 * MAX_STAGES);
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + 2 * MAX_STAGES + 1);
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int nt = blockIdx.y;
-    const int ci_tile = p.kwin ? nt : blockIdx.x;
-    const int tap = blockIdx.z / p.splitK, split = blockIdx.z % p.splitK;
     const int n_tile = p.n_tile;
+    const int ci_tile = p.kwin ? nt * n_tile / BLOCK_CI : blockIdx.x;
+    const int tap = blockIdx.z / p.splitK, split = blockIdx.z % p.splitK;
     const int kb0 = split * p.kb_per_split;
     int kb1 = kb0 + p.kb_per_split;
     if (kb1 > p.KBp) kb1 = p.KBp;
@@ -78,12 +75,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
             mbar_init(full(s), 2 * GROUP_THREADS);      // both producer groups (x tile + dY tile) arrive
-            mbar_init(empty(s), 1);
+            mbar_init(empty(s), CONSUMER_THREADS);
         }
-        mbar_init(accum_full, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) tmem_alloc(smem_u32(tmem_slot), 256);
     if (p.pre_scale) {
         for (int c = threadIdx.x; c < BLOCK_CI; c += NUM_THREADS) {
             const int ch = ci_tile * BLOCK_CI + c;
@@ -91,118 +86,85 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             s_shift[c] = ch < p.Cin ? p.pre_shift[ch] : 0.f;
         }
     }
-    // chunks of the A operand beyond the last live input channel are never produced: zero them once
-    for (int i = threadIdx.x; i < S * 2 * A_BYTES / 16; i += NUM_THREADS) {
-        const int st_ = i / (2 * A_BYTES / 16), r_ = i % (2 * A_BYTES / 16);
-        st_shared_v4(base + (uint32_t)st_ * stage_bytes + r_ * 16, 0.f, 0.f, 0.f, 0.f);
-    }
+    // channel chunks beyond the last live input / output channel are never produced: zero every stage once
+    for (int i = threadIdx.x; i < S * stage_bytes / 16; i += NUM_THREADS) st_shared_v4(base + i * 16, 0.f, 0.f, 0.f, 0.f);
     fence_proxy_async();
-    tc_fence_before();
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 1) {
-        // MMA issuer.  Whole warp runs the loop (warp-uniform control flow keeps the descriptors in uniform registers and
-        // lets the compiler emit back-to-back UTCHMMA); one elected lane issues.  Descriptors advance by constants -- the
-        // round-1 loop rebuilt 16 descriptors per k-block from addresses and paid ~300 issue-warp instructions per
-        // k-block (see conv_tc.cu), which is what held every wgrad layer at 2.2-3.7x its MMA bound.
-        // 2 MMAs per k-group instead of 3: the dY_lo chunks follow the dY_hi chunks in the stage, so one instruction with
-        // N = 32*nchunk + n_tile computes x_hi^T * [dY_hi ; dY_lo]; the epilogue adds the column blocks [0,n_tile) and
-        // [32*nchunk, 32*nchunk+n_tile).  Wider tiles (n_tile > 128): three plain products per k-group.
-        if (p.legacy) {
-        if (lane == 0) {
-            // 2 MMAs per k-group instead of 3 (a tcgen05.mma with M=128, K=8 costs ~120 cycles whatever N is): the dY_lo
-            // chunks follow the dY_hi chunks in the stage, so one instruction with N = 32*nchunk + n_tile computes
-            // x_hi^T * [dY_hi ; dY_lo]; the epilogue adds the column blocks [0,n_tile) and [32*nchunk, 32*nchunk+n_tile).
-            const int nchunk_b = (n_tile + 31) >> 5;
-            const uint32_t idesc = make_idesc(BLOCK_CI, n_tile, 1, 1);
-            const uint32_t idesc2 = make_idesc(BLOCK_CI, nchunk_b * 32 + n_tile, 1, 1);
-            const bool stack = n_tile <= 128;          // wider tiles: three plain products per k-group
+    if (warp < CONSUMER_THREADS / 32) {
+        // ---- consumers: two warpgroups, input channels [64 wg, 64 wg + 64) of the tile; 3xTF32 per k8 step, small
+        //      cross terms first; a stage is released as soon as its wgmma group has completed (the other warpgroup keeps
+        //      the tensor cores busy meanwhile)
+        const int wg = warp >> 2;
+        const uint32_t b_off = 2 * A_BYTES;
+        const uint32_t bl_off = b_off + (uint32_t)p.b_bytes;
+        auto consume = [&](auto NT) {
+            constexpr int N = decltype(NT)::value;
+            float acc[N / 2];
+#pragma unroll
+            for (int i = 0; i < N / 2; ++i) acc[i] = 0.f;
             int s = 0;
             uint32_t ph = 0;
             for (int it = 0; it < nkb; ++it) {
                 mbar_wait(full(s), ph);
-                tc_fence_after();
-                const uint32_t a_hi = base + (uint32_t)s * stage_bytes, a_lo = a_hi + A_BYTES;
-                const uint32_t b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + (uint32_t)nchunk_b * CHUNK_BYTES;
+                wgmma_fence();
+                const uint32_t st = base + (uint32_t)s * stage_bytes;
+                const uint32_t a_hi = st + (uint32_t)wg * 8u * CORE_SBO;
 #pragma unroll
                 for (int kg = 0; kg < BLOCK_KP / 8; ++kg) {
-                    const uint64_t dah = make_desc_mn(a_hi + kg * 1024, CHUNK_BYTES), dal = make_desc_mn(a_lo + kg * 1024, CHUNK_BYTES);
-                    const uint64_t dbh = make_desc_mn(b_hi + kg * 1024, CHUNK_BYTES), dbl = make_desc_mn(b_lo + kg * 1024, CHUNK_BYTES);
-                    if (p.precision == 0 && stack) {
-                        umma_tf32(tmem_base, dah, dbh, idesc2, (it | kg) != 0);   // x_hi * [dY_hi ; dY_lo]
-                        umma_tf32(tmem_base, dal, dbh, idesc, 1);                 // x_lo * dY_hi
-                    } else if (p.precision == 0) {
-                        umma_tf32(tmem_base, dal, dbh, idesc, (it | kg) != 0);
-                        umma_tf32(tmem_base, dah, dbl, idesc, 1);
-                        umma_tf32(tmem_base, dah, dbh, idesc, 1);
+                    const uint32_t ko = (uint32_t)kg * 256u;
+                    const uint64_t dah = make_desc_core(a_hi + ko, 128, CORE_SBO), dal = make_desc_core(a_hi + A_BYTES + ko, 128, CORE_SBO);
+                    const uint64_t dbh = make_desc_core(st + b_off + ko, 128, CORE_SBO), dbl = make_desc_core(st + bl_off + ko, 128, CORE_SBO);
+                    const uint32_t accumulate = (it | kg) != 0;
+                    if (p.precision != 0) {
+                        Wgmma<N>::mma(acc, dah, dbh, accumulate);
                     } else {
-                        umma_tf32(tmem_base, dah, dbh, idesc, (it | kg) != 0);
+                        Wgmma<N>::mma(acc, dal, dbh, accumulate);
+                        Wgmma<N>::mma(acc, dah, dbl, 1);
+                        Wgmma<N>::mma(acc, dah, dbh, 1);
                     }
                 }
-                umma_commit(empty(s));
+                wgmma_commit();
+                wgmma_wait<0>();
+                mbar_arrive(empty(s));
                 if (++s == S) { s = 0; ph ^= 1; }
             }
-            umma_commit(accum_full);
-        }
-        } else {
-        const int nchunk_b = (n_tile + 31) >> 5;
-        const uint32_t idesc = make_idesc(BLOCK_CI, n_tile, 1, 1);
-        const uint32_t idesc2 = make_idesc(BLOCK_CI, nchunk_b * 32 + n_tile, 1, 1);
-        const int mode = p.precision != 0 ? 2 : (n_tile <= 128 ? 0 : 1);
-        const uint64_t dA0 = make_desc_mn(base, CHUNK_BYTES);                     // x_hi of stage 0, k-group 0
-        const uint64_t oAlo = (uint64_t)(A_BYTES >> 4), oBhi = (uint64_t)((2 * A_BYTES) >> 4);
-        const uint64_t oBlo = oBhi + (uint64_t)((nchunk_b * CHUNK_BYTES) >> 4), stage_step = (uint64_t)(stage_bytes >> 4);
-        constexpr uint64_t KG = 1024 >> 4;                                         // one k-group = 8 pixel rows = 1024 B
-        const bool leader = elect_one();
-        int s = 0;
-        uint32_t ph = 0;
-        uint64_t d = dA0;
-        uint32_t bfull = full(0), bempty = empty(0);
-        for (int it = 0; it < nkb; ++it) {
-            mbar_wait(bfull, ph);
-            tc_fence_after();
-            if (leader) {
-                const uint64_t dah = d, dal = d + oAlo, dbh = d + oBhi, dbl = d + oBlo;
-                const uint32_t first = it != 0;
-                if (mode == 0) {
-                    umma_tf32(tmem_base, dah, dbh, idesc2, first);                // x_hi * [dY_hi ; dY_lo]
-                    umma_tf32(tmem_base, dal, dbh, idesc, 1);                     // x_lo * dY_hi
+            wgmma_wait<0>();
+            wgmma_fence_operands(acc);
+            // ---- epilogue: accumulator row = input channel, column = output channel; partial [split][tap][ci][co]
+            const int taps = p.KH * p.KW;
+            const bool ovec = (p.Cout & 1) == 0 && ((((uintptr_t)p.part) & 7) == 0) && (n_tile & 1) == 0;
 #pragma unroll
-                    for (int kg = 1; kg < BLOCK_KP / 8; ++kg) {
-                        umma_tf32(tmem_base, dah + kg * KG, dbh + kg * KG, idesc2, 1);
-                        umma_tf32(tmem_base, dal + kg * KG, dbh + kg * KG, idesc, 1);
+            for (int i = 0; i < 2; ++i) {
+                const int ci = ci_tile * BLOCK_CI + wg * 64 + (warp & 3) * 16 + (lane >> 2) + 8 * i;
+                if (ci >= p.Cin) continue;
+                float *prow = p.kwin ? p.part + (((long long)split * taps + tap) * p.Cin + ci) * p.kwin + (nt * n_tile) % p.kwin
+                                     : p.part + (((long long)split * taps + tap) * p.Cin + ci) * p.Cout + (long long)nt * n_tile;
+                const int ccap = p.kwin ? n_tile : p.Cout - nt * n_tile;     // live columns of this tile
+#pragma unroll
+                for (int j = 0; j < N / 8; ++j) {
+                    const int col = 8 * j + (lane & 3) * 2;
+                    const float v0 = acc[4 * j + 2 * i], v1 = acc[4 * j + 2 * i + 1];
+                    if (ovec && col + 1 < ccap) {
+                        *reinterpret_cast<float2 *>(prow + col) = make_float2(v0, v1);
+                    } else {
+                        if (col < ccap) prow[col] = v0;
+                        if (col + 1 < ccap) prow[col + 1] = v1;
                     }
-                } else if (mode == 1) {
-                    umma_tf32(tmem_base, dal, dbh, idesc, first);
-                    umma_tf32(tmem_base, dah, dbl, idesc, 1);
-                    umma_tf32(tmem_base, dah, dbh, idesc, 1);
-#pragma unroll
-                    for (int kg = 1; kg < BLOCK_KP / 8; ++kg) {
-                        umma_tf32(tmem_base, dal + kg * KG, dbh + kg * KG, idesc, 1);
-                        umma_tf32(tmem_base, dah + kg * KG, dbl + kg * KG, idesc, 1);
-                        umma_tf32(tmem_base, dah + kg * KG, dbh + kg * KG, idesc, 1);
-                    }
-                } else {
-                    umma_tf32(tmem_base, dah, dbh, idesc, first);
-#pragma unroll
-                    for (int kg = 1; kg < BLOCK_KP / 8; ++kg) umma_tf32(tmem_base, dah + kg * KG, dbh + kg * KG, idesc, 1);
                 }
-                umma_commit(bempty);
-                if (it == nkb - 1) umma_commit(accum_full);
             }
-            __syncwarp();
-            d += stage_step; bfull += 8u; bempty += 8u;
-            if (++s == S) { s = 0; ph ^= 1; d = dA0; bfull = full(0); bempty = empty(0); }
+        };
+        switch (n_tile) {
+            case 16: consume(std::integral_constant<int, 16>()); break;
+            case 32: consume(std::integral_constant<int, 32>()); break;
+            case 48: consume(std::integral_constant<int, 48>()); break;
+            default: consume(std::integral_constant<int, 64>()); break;
         }
-        if (nkb == 0 && leader) umma_commit(accum_full);      // empty split: release the epilogue (it writes zeros)
-        }   // lean issue loop
-    } else if (warp >= 2) {
+    } else {
         // 8 warps per group (round 1 ran 4 with two pixel rows per thread: ~9 cycles between a warp's instructions at
         // 2.5 warps per scheduler made the producers, not the tensor pipe, set the k-block time): one pixel row of the
         // 32-pixel k-block per thread, 4 sixteen-byte units (one per 32-channel chunk).
-        const int pt = threadIdx.x - 64;
+        const int pt = threadIdx.x - CONSUMER_THREADS;
         const int grp = pt >> 8;                   // group 0 produces the x (A) tiles, group 1 the dY (B) tiles
         const int t = pt & 255;
         const int unit = t & 7;                    // 16-byte unit of the 128-byte row
@@ -210,9 +172,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
         constexpr bool AFF = PRE >= 2;
         constexpr bool RELU = (PRE & 1) != 0;
         constexpr int NU = 4;                      // units per thread per k-block
+        // K-major core-matrix tiles: element (row = channel, k = pixel) at (row / 8) * CORE_SBO + (k / 4) * 128 +
+        // (row % 8) * 16 + (k % 4) * 4.  A thread holds 4 consecutive channels of one pixel: 4 scalar stores, which the
+        // 16-byte pad of CORE_SBO spreads over all 32 banks across the warp.
         uint32_t roff[NU];
 #pragma unroll
-        for (int i = 0; i < NU; ++i) roff[i] = (uint32_t)i * CHUNK_BYTES + mn_swizzle_off(r0, unit);
+        for (int i = 0; i < NU; ++i)
+            roff[i] = (uint32_t)(i * 4 + (unit >> 1)) * CORE_SBO + (uint32_t)(r0 >> 2) * 128u + (uint32_t)(unit & 1) * 64u +
+                      (uint32_t)(r0 & 3) * 4u;
 
         // hi/lo split + swizzled stores of up to 8 units (4 chunks x 2 rows); only `nlive` chunks are written
         // (the A regions were zeroed once, so dead channel chunks stay zero)
@@ -228,8 +195,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
                         hi[e] = hh;
                         lo[e] = a - hh;
                     }
-                    st_shared_v4(t_hi + roff[i], hi[0], hi[1], hi[2], hi[3]);
-                    st_shared_v4(t_lo + roff[i], lo[0], lo[1], lo[2], lo[3]);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        st_shared_f32(t_hi + roff[i] + 16u * e, hi[e]);
+                        st_shared_f32(t_lo + roff[i] + 16u * e, lo[e]);
+                    }
                 }
             }
         };
@@ -347,19 +317,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
                 }
             }
         } else {
-            // ------------------------------ dY tiles (B operand): ceil(n_tile/32) chunks of output channels ------
+            // ------------------------------ dY tiles (B operand): ceil(n_tile/32) <= 2 chunks of output channels ---
             const int dys = (int)p.dys;
             const int nchunk = (n_tile + 31) >> 5;
             const int cb = nt * n_tile + unit * 4;
             const float *__restrict__ dg = p.dy;
-            // wide tiles (n_tile > 128: 5..8 chunks) are produced in two passes of 4 chunks per k-block; j counts passes
-            const int npass = (nchunk + 3) >> 2;
-            auto load_d = [&](int j, F4(&v)[NU]) {
-                const int it = npass == 2 ? (j >> 1) : j, pass = npass == 2 ? (j & 1) : 0;
+            auto load_d = [&](int it, F4(&v)[NU]) {
                 const int kb = kb0 + it;
 #pragma unroll
                 for (int i = 0; i < NU; ++i) {
-                    const int chunk = pass * 4 + i;
+                    const int chunk = i;
                     const int m = kb * BLOCK_KP + r0;
                     const int c = cb + chunk * 32;
                     const bool live = chunk < nchunk && m < p.M && c < p.Cout;
@@ -384,80 +351,31 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             };
             int ds_s = 0;
             uint32_t ds_ph = 0;
-            auto store_d = [&](int j, F4(&v)[NU]) {
-                const int pass = npass == 2 ? (j & 1) : 0;
+            auto store_d = [&](F4(&v)[NU]) {
                 const int s = ds_s;
-                if (pass == 0) mbar_wait(empty(s), ds_ph ^ 1);
-                const uint32_t t_hi = base + (uint32_t)s * stage_bytes + 2 * A_BYTES + (uint32_t)pass * 4u * CHUNK_BYTES;
-                split_store(t_hi, t_hi + (uint32_t)nchunk * CHUNK_BYTES, v, nchunk - pass * 4);
-                if (pass == npass - 1) {
-                    fence_proxy_async();
-                    mbar_arrive(full(s));
-                    if (++ds_s == S) { ds_s = 0; ds_ph ^= 1; }
-                }
+                mbar_wait(empty(s), ds_ph ^ 1);
+                const uint32_t t_hi = base + (uint32_t)s * stage_bytes + 2 * A_BYTES;
+                split_store(t_hi, t_hi + (uint32_t)p.b_bytes, v, nchunk);
+                fence_proxy_async();
+                mbar_arrive(full(s));
+                if (++ds_s == S) { ds_s = 0; ds_ph ^= 1; }
             };
             F4 va[NU], vb[NU];
-            const int nj = nkb * npass;
+            const int nj = nkb;
             int it = 0;
             if (it < nj) load_d(it, va);
             for (; it < nj; it += 2) {
                 const bool more = it + 1 < nj;
                 if (more) load_d(it + 1, vb);
-                store_d(it, va);
+                store_d(va);
                 if (more) {
                     if (it + 2 < nj) load_d(it + 2, va);
-                    store_d(it + 1, vb);
+                    store_d(vb);
                 }
             }
         }
 
-        // ---- epilogue: TMEM lane = input channel, columns = output channels (first 4 warps of each group: one per
-        //      TMEM lane quarter; group 0 takes the low half of the columns, group 1 the high half)
-        if (t < 128) {
-        mbar_wait(accum_full, 0);
-        tc_fence_after();
-        const int q = warp & 3;
-        const int ci = ci_tile * BLOCK_CI + q * 32 + lane;
-        const int half = n_tile >> 1;
-        const int col0 = grp * half;
-        const int taps = p.KH * p.KW;
-        float *prow = p.kwin ? p.part + (((long long)split * taps + tap) * p.Cin + (ci < p.Cin ? ci : 0)) * n_tile
-                             : p.part + (((long long)split * taps + tap) * p.Cin + (ci < p.Cin ? ci : 0)) * p.Cout + (long long)nt * n_tile;
-        const bool ovec = (p.Cout & 3) == 0 && ((((uintptr_t)p.part) & 15) == 0);
-        const int lo_col = ((n_tile + 31) >> 5) * 32;       // first accumulator column of the x_hi * dY_lo block
-        for (int cc = 0; cc < half; cc += 8) {
-            uint32_t r[8];
-            tmem_ld8(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(col0 + cc), r);
-            if (p.precision == 0 && n_tile <= 128) {
-                uint32_t r2[8];
-                tmem_ld8(tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(lo_col + col0 + cc), r2);
-                tmem_ld_wait();
-#pragma unroll
-                for (int e = 0; e < 8; ++e) r[e] = __float_as_uint(__uint_as_float(r[e]) + __uint_as_float(r2[e]));
-            } else {
-                tmem_ld_wait();
-            }
-            if (ci < p.Cin) {
-                const int cbase = nt * n_tile + col0 + cc;
-#pragma unroll
-                for (int e4 = 0; e4 < 8; e4 += 4) {
-                    if (ovec && cbase + e4 + 3 < p.Cout) {
-                        *reinterpret_cast<float4 *>(prow + col0 + cc + e4) =
-                            make_float4(nkb ? __uint_as_float(r[e4]) : 0.f, nkb ? __uint_as_float(r[e4 + 1]) : 0.f,
-                                        nkb ? __uint_as_float(r[e4 + 2]) : 0.f, nkb ? __uint_as_float(r[e4 + 3]) : 0.f);
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 4; ++e)
-                            if (cbase + e4 + e < p.Cout) prow[col0 + cc + e4 + e] = nkb ? __uint_as_float(r[e4 + e]) : 0.f;
-                    }
-                }
-            }
-        }
-        }
     }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc(tmem_base, 256);
 }
 
 // dW[co,ci,kh,kw] (arbitrary strides) = sum_split part[split][tap][ci][co]; fixed summation order -> deterministic
@@ -500,13 +418,9 @@ __global__ void __launch_bounds__(256) wgrad_reduce_grouped_kernel(const float *
 
 }  // namespace
 
-// N tile of the wgrad kernels (their shared-memory plan holds <= 128 output channels per CTA)
+// N tile of the wgrad kernels: <= MAX_N output channels per CTA (the consumers' register accumulator)
 static int wgrad_n_tile(int Cout) {
-    static int cap = 0;
-    if (!cap) {
-        const char *e = getenv("BTS_B200_WGRAD_WIDE");        // 0: 128-wide tiles (hi/lo stacked), default: up to 256
-        cap = (e && e[0] == '0') ? 128 : MAX_N;
-    }
+    const int cap = MAX_N;
     int n = (Cout + 15) / 16 * 16;
     if (n > cap) {
         const int tiles = (n + cap - 1) / cap;
@@ -515,7 +429,6 @@ static int wgrad_n_tile(int Cout) {
     return n;
 }
 
-int bts_issue_legacy();      // conv_tc.cu: 1 = round-1 MMA issue loops (fallback switch)
 
 // narrow-output 3x3 layers use the shifted-dY kernel (wgrad2_tc.cu)
 bool bts_wgrad2_eligible(int Cout, int KH, int KW, int stride, long long Mq);
@@ -540,7 +453,7 @@ extern "C" int bts_conv_wgrad_plan(int B, int Hout, int Wout, int Cin, int Cout,
     const int n_tile = wgrad_n_tile(Cout);
     const long long tiles = (long long)((Cin + BLOCK_CI - 1) / BLOCK_CI) * ((Cout + n_tile - 1) / n_tile) * KH * KW;
     const int sms = bts_num_sms();
-    // split-K so that the CTA count fills whole waves of the SMs (a 297-CTA grid on 148 SMs wastes a third of the
+    // split-K so that the CTA count fills whole waves of the SMs (a grid of 1.5 waves wastes a third of the
     // time in a 1-CTA tail): among splits giving <= 4 waves pick the best wave efficiency, ties -> more CTAs
     long long max_split = (KBp + 15) / 16;                    // at least 16 k-blocks (512 px) per CTA
     if (max_split < 1) max_split = 1;
@@ -582,7 +495,6 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     p.M = (int)M;
     p.n_tile = wgrad_n_tile(Cout);
     p.kwin = 0;
-    p.legacy = bts_issue_legacy();
     p.part = workspace; p.splitK = splitK;
     p.KBp = (int)((M + BLOCK_KP - 1) / BLOCK_KP);
     p.kb_per_split = (p.KBp + splitK - 1) / splitK;
@@ -606,7 +518,8 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     }
     {
         const int nchunk = (p.n_tile + 31) / 32;
-        p.stage_bytes = 2 * A_BYTES + 2 * nchunk * CHUNK_BYTES;
+        p.b_bytes = nchunk * 4 * (int)CORE_SBO;
+        p.stage_bytes = 2 * A_BYTES + 2 * p.b_bytes;
         p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
         if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
         if (p.stages < 2) return BTS_EINVAL;
@@ -657,11 +570,10 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
 // (width, cpg, KH, KW).  Only the diagonal 128 x 128 channel blocks are computed (one CTA per block, tap and split),
 // the reduce kernel extracts every group's cpg x cpg sub-block.  Requires bts_conv_group_window(width, cpg) == 128.
 extern "C" int bts_conv_group_window(int width, int cpg);
-int bts_issue_legacy();
 
 static long long wgrad_grouped_split(long long M, int width, int taps) {
     const long long KBp = (M + BLOCK_KP - 1) / BLOCK_KP;
-    const long long tiles = (long long)(width / 128) * taps;
+    const long long tiles = (long long)(width / MAX_N) * taps;       // CTAs per split: the grid of bts_conv_wgrad_grouped
     const int sms = bts_num_sms();
     long long max_split = (KBp + 15) / 16;
     if (max_split < 1) max_split = 1;
@@ -707,8 +619,7 @@ extern "C" int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, 
     if (p.Hout < 1 || p.Wout < 1 || M > 0x7ffffff0LL) return BTS_EINVAL;
     if ((long long)B * Hs * Ws * x_pixel_stride >= 0x7fffffffLL || M * dy_pixel_stride >= 0x7fffffffLL) return BTS_EINVAL;
     p.M = (int)M;
-    p.n_tile = 128; p.kwin = 128;
-    p.legacy = bts_issue_legacy();
+    p.n_tile = MAX_N; p.kwin = 128;
     p.part = workspace; p.splitK = splitK;
     p.KBp = (int)((M + BLOCK_KP - 1) / BLOCK_KP);
     p.kb_per_split = (p.KBp + splitK - 1) / splitK;
@@ -716,11 +627,12 @@ extern "C" int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, 
     p.dy_vec = bts_aligned16(dy) && (dy_pixel_stride % 4 == 0);
     p.precision = precision;
     const int taps = KH * KW;
-    p.stage_bytes = 2 * A_BYTES + 2 * 4 * CHUNK_BYTES;
+    p.b_bytes = 2 * 4 * (int)CORE_SBO;
+    p.stage_bytes = 2 * A_BYTES + 2 * p.b_bytes;
     p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     const int smem = p.stages * p.stage_bytes + 2 * BLOCK_CI * 4 + 256 + 1024;
-    dim3 grid(1, width / 128, taps * splitK);
+    dim3 grid(1, width / MAX_N, taps * splitK);
     if (grid.z > 65535) return BTS_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t err = cudaSuccess;

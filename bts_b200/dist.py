@@ -3,7 +3,7 @@ step -- a mean all-reduce of the gradient vector -- plus the rank-0 broadcast of
 gets from DistributedDataParallel (bts_main.py:352: C1 + C3 in SURVEY 2.5).
 
 The drop-in boundary is the module, so an unchanged bts_main.py keeps using torch's DDP.  `FlatGradReducer` +
-`FlatBufferBroadcaster` are the B200-native alternative that bench.py uses for N > 1 (`--reducer flat`, the default;
+`FlatBufferBroadcaster` are the native alternative that bench.py uses for N > 1 (`--reducer flat`, the default;
 `--reducer ddp` runs torch's DDP exactly as bts_main.py does): one all-reduce over a single flat buffer after backward.  Works with the gloo backend on CPU tensors, which is how
 tests/test_dist_cpu.py covers it.
 """
@@ -27,9 +27,8 @@ class FlatGradReducer:
     """ONE mean all-reduce of the whole gradient vector per step over a single persistent flat fp32 buffer.
 
     DDP buckets the 187 MB (DenseNet-161) gradient into 25 MB pieces and overlaps their all-reduces with the backward
-    pass; on B200 every conv kernel is a persistent one-CTA-per-SM grid, so NCCL's reduction kernels cannot run beside
-    them and the "overlap" serialises piecemeal (measured round 1: +11 ms/step at 8 GPUs).  Over NVSwitch the whole
-    vector crosses the wire in ~0.5 ms (measured bus bandwidth 725 GB/s), so the B200-native schedule is the simple one:
+    pass; every conv kernel here is a persistent one-CTA-per-SM grid, so NCCL's reduction kernels cannot run beside
+    them and the "overlap" serialises piecemeal.  The schedule is therefore the simple one:
     finish backward, gather the gradients into the flat buffer with one multi-tensor copy, one NCCL all-reduce (AVG),
     and let the optimizer read the flat views.  Parameters without a gradient contribute zeros (like DDP with
     find_unused_parameters=True, bts_main.py:352).  Works with gloo on CPU tensors (tests/test_dist_cpu.py)."""

@@ -8,7 +8,7 @@ kernels and two cuDNN convs forward, and the mirror image plus one `add` per con
   forward   one NHWC slab holds every feature; each layer's 3x3 conv writes its 48 channels straight into its slice.
             Batch statistics of a feature are reduced ONCE, when it is produced (every later BN re-reads the same
             channel: same mean/var, different gamma/beta).  BN-apply + ReLU never run as kernels -- they are the
-            A-operand prologue of the consuming tcgen05 conv (scale/shift per channel).
+            A-operand prologue of the consuming wgmma conv (scale/shift per channel).
   backward  one gradient slab accumulates the concat fan-out in place (the BN+ReLU backward kernel writes `+=` into
             its channel range), dgrad / wgrad run on the tensor-core engine with the same fused prologue.
 
@@ -118,10 +118,9 @@ def bn_backward_correct(x, K, out):
     _lib.count()
 
 
-# BatchNorm-backward sums reduced in the dgrad epilogue (bts_conv_fwd_bnbwd) instead of a separate pass.  Measured on B200
-# (profiles/r02_*): the four epilogue warps already pace the short-K dgrads, and the extra strided reads of x + the
-# per-channel parameters doubled their time (dgrad 20.0 -> 33.4 ms per K16 step against 7.4 ms of reduce passes saved), so the
-# separate streaming reduce pass is the default; the fused form stays available (and tested) for long-K layers.
+# BatchNorm-backward sums reduced in the dgrad epilogue (bts_conv_fwd_bnbwd) instead of a separate pass.  The epilogue
+# already paces the short-K dgrads, and the fused form adds strided reads of x and of the per-channel parameters to it, so
+# the separate streaming reduce pass is the default; the fused form stays available (and tested) for long-K layers.
 EPI_BNBWD = os.environ.get("BTS_B200_EPI_BNBWD", "0") == "1"
 
 

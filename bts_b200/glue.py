@@ -1,6 +1,6 @@
 """Composable fused autograd units for the BTS decoder and the encoder's non-dense-block stages (SURVEY 8a rows a5-a10,
 a11 transitions/stem).  The reference (torch-eager, pytorch/bts.py:196-266) runs every BatchNorm, ReLU, ELU, nearest
-up-sample and torch.cat as its own ATen/cuDNN kernel, forward and backward; here they are either folded into the tcgen05
+up-sample and torch.cat as its own ATen/cuDNN kernel, forward and backward; here they are either folded into the wgmma
 conv engine (ELU in the epilogue, ReLU / BN-apply + ReLU in the A-operand prologue, the x2 up-sample in the im2col map) or
 run as one of the streaming NHWC kernels of csrc/elem.cu / csrc/bn.cu:
 

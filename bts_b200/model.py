@@ -1,11 +1,11 @@
-"""Host-side mirror of the reference's module surface (pytorch/bts.py) over the B200 kernels.
+"""Host-side mirror of the reference's module surface (pytorch/bts.py) over the native kernels.
 
 Same class names, constructor arguments, forward signatures, 5-tuple output and -- the checkpoint wire
 format -- the same state_dict keys and shapes (SURVEY.md Appendix C), so the reference's bts_main.py /
 bts_test.py import this as `bts` unchanged.  The arithmetic underneath is ours:
-  * plane heads + LPG + /max_depth + nearest down-sample: one fused sm_100a kernel each way (ops.plane_head_lpg)
+  * plane heads + LPG + /max_depth + nearest down-sample: one fused sm_90a kernel each way (ops.plane_head_lpg)
   * silog loss: two streaming kernels (ops.silog)
-  * convolutions: the tcgen05 implicit-GEMM engine (bts_b200.conv) where enabled, cuDNN otherwise (scaffold)
+  * convolutions: the wgmma implicit-GEMM engine (bts_b200.conv)
 Reference lines are cited per class.
 """
 import math
@@ -54,7 +54,7 @@ def _require_cuda_fp32(x, what):
 
 
 class Conv2dTC(nn.Conv2d):
-    """nn.Conv2d whose forward/dgrad run on the tcgen05 engine.  It stays an nn.Conv2d subclass so that
+    """nn.Conv2d whose forward/dgrad run on the wgmma engine.  It stays an nn.Conv2d subclass so that
     weights_init_xavier (bts_main.py:338), state_dict keys and optimizer groups behave exactly as in the reference."""
 
     def forward(self, x):
@@ -126,7 +126,7 @@ def _bottleneck_class():
 
     class BottleneckTC(Bottleneck):
         """torchvision ResNet / ResNeXt bottleneck [1x1 -> BN -> ReLU -> (grouped) 3x3 -> BN -> ReLU -> 1x1 -> BN -> +id ->
-        ReLU]: every conv on the tcgen05 engine (the grouped 3x3 as a block-diagonal operator), BN(+ReLU) and the
+        ReLU]: every conv on the wgmma engine (the grouped 3x3 as a block-diagonal operator), BN(+ReLU) and the
         BN + residual + ReLU tail on our streaming kernels; parameters / buffers / state_dict untouched."""
 
         def forward(self, x):
@@ -365,7 +365,7 @@ class bts(nn.Module):
 
     def _forward_fused(self, features, focal):
         """bts.forward (reference pytorch/bts.py:196-266) over the fused units of bts_b200/glue.py: no ATen BatchNorm /
-        ReLU / ELU / interpolate / cat kernels; every conv (fwd, dgrad, wgrad) on the tcgen05 engine."""
+        ReLU / ELU / interpolate / cat kernels; every conv (fwd, dgrad, wgrad) on the wgmma engine."""
         from . import glue as G
         skip0, skip1, skip2, skip3 = features[0], features[1], features[2], features[3]
         md = self.params.max_depth

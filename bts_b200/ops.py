@@ -1,7 +1,7 @@
 """torch.autograd bindings of the C-ABI kernels (include/bts_b200.h).
 
 PyTorch is plumbing here: device memory, the current stream, autograd bookkeeping.  Every op launches
-hand-written sm_100a kernels from libbts_b200.so through ctypes with raw device pointers; there is no eager
+hand-written sm_90a kernels from libbts_b200.so through ctypes with raw device pointers; there is no eager
 or CPU fallback -- non-CUDA inputs raise.
 """
 import ctypes
@@ -24,7 +24,7 @@ def _stream():
 def _need_cuda(*ts):
     for t in ts:
         if t is not None and not t.is_cuda:
-            raise RuntimeError("bts_b200 ops run on CUDA (sm_100a) tensors only; got a %s tensor -- "
+            raise RuntimeError("bts_b200 ops run on CUDA (sm_90a) tensors only; got a %s tensor -- "
                                "there is no CPU fallback" % t.device.type)
 
 

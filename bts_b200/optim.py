@@ -4,7 +4,7 @@
 poly-LR loop `for g in optimizer.param_groups: g['lr'] = ...` works unchanged), same `state` / `state_dict()` layout
 (`step`, `exp_avg`, `exp_avg_sq` per parameter: checkpoints written by either optimizer load into the other) -- whose
 `step()` is ONE multi-tensor CUDA kernel (csrc/optim.cu) over every parameter of every group, followed by ONE launch that
-re-packs every cached conv operator of the tcgen05 engine (hi/lo split, swizzled tiles, forward and transposed) instead of
+re-packs every cached conv operator of the wgmma engine (hi/lo split, swizzled tiles, forward and transposed) instead of
 one pack launch per layer at the next forward pass (394 launches per step for DenseNet-161 + decoder).
 """
 import ctypes

@@ -1,4 +1,4 @@
-/* bts_b200 -- C ABI of the B200-native BTS hot path (libbts_b200.so).
+/* bts_b200 -- C ABI of the GPU-native BTS hot path (libbts_b200.so, built for the H100: sm_90a).
  *
  * This is the native boundary underneath the Python module surface `bts` (BtsModel / encoder / bts /
  * local_planar_guidance / reduction_1x1 / silog_loss, reference pytorch/bts.py).  The reference's only
@@ -32,7 +32,7 @@ extern "C" {
 #define BTS_EINVAL (-1)   /* bad argument (null pointer, non-positive size, unsupported upratio) */
 #define BTS_EALIGN (-2)   /* pointer not 16-byte aligned where the kernel needs it */
 
-/* library / build identification: returns e.g. 100 for sm_100a; writes a short version string */
+/* library / build identification: returns the target architecture (90 for sm_90a); writes a short version string */
 int bts_version(char *buf, int buflen);
 
 /* ---- Local planar guidance --------------------------------------------------------------------
@@ -86,8 +86,8 @@ int bts_plane_head_fwd(const float *c3, float *plane_out, float *scaled, float *
 int bts_plane_head_bwd(const float *d_scaled, const float *d_ds, const float *c3, float *dc3,
                        float max_depth, int ds_stride, int B, int h, int w, int r, void *stream);
 
-/* ---- tcgen05 implicit-GEMM convolution (pytorch/bts.py:51-80,153-194; torchvision dense/bottleneck layers) ----
- * NHWC activations, fp32 in / fp32 out, parity-grade 3xTF32 on the 5th-gen tensor cores (precision=0) or
+/* ---- wgmma implicit-GEMM convolution (pytorch/bts.py:51-80,153-194; torchvision dense/bottleneck layers) ----
+ * NHWC activations, fp32 in / fp32 out, parity-grade 3xTF32 on the Hopper tensor cores (precision=0) or
  * single-pass TF32 (precision=1, labelled fast mode, not parity).
  *   out[p,co] = act( sum_{tap,ci} pre(x[p (+) tap, ci]) * w[co,ci,tap] )
  *   pre : x*pre_scale[ci]+pre_shift[ci] (folded BatchNorm; both NULL to skip), then ReLU if pre_relu;
@@ -135,17 +135,15 @@ int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int
                     const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
                     int act, int precision, double *stat_sum, double *stat_sumsq, int flags, void *stream);
 /* Staging of the activation tiles of bts_conv_fwd*: 0 = the producer warps load them (LDG + hi/lo split in registers),
- * 1 = TMA im2col loads (cp.async.bulk.tensor -> UTMALDG.4D.IM2COL; zero padding by out-of-bounds fill) land the raw tile in
+ * 1 = TMA im2col loads (cp.async.bulk.tensor im2col; zero padding by out-of-bounds fill) land the raw tile in
  * shared memory as the A_hi operand and the producers only derive A_lo in place -- used for stride-1, non-up-sampled layers
  * whose K channels are a multiple of 32 and whose rows are 16-byte aligned, every other layer keeps mode 0 automatically.
  * (2, 3: bring-up variants.)  Process-wide setting. */
 int bts_conv_set_tma(int mode);
 int bts_conv_get_tma(void);
-/* MMA issue loops of the three tensor-core kernels: 1 (default) = whole-warp loop with one elected lane, one barrier per stage,
- * incrementally advanced descriptors; 0 = the round-1 single-lane loops, kept as a bring-up fallback.  Process-wide. */
-int bts_conv_set_issue_mode(int lean);
-/* activation-producer groups of the conv engine (4 warps each): 0 / 4 = four groups without register prefetch wherever the
- * operand ring has >= 4 stages (default), 2 = always two groups with one k-block of register prefetch (round-1 layout). */
+/* activation-producer groups of the conv engine (4 warps each): 0 / 4 = four groups without register prefetch on narrow
+ * tiles (<= 48 output channels) whose operand ring has >= 4 stages (default), 2 = always two groups with one k-block of
+ * register prefetch. */
 int bts_conv_set_producer_groups(int groups);
 /* Tuning / bring-up switches of the narrow-output wgrad (csrc/wgrad2_tc.cu).  set_tma(0): the producers load the operands
  * from global memory (round-1 path) instead of the TMA landing ring; set_min_pixels(n): smallest map (input pixels) routed to
@@ -153,7 +151,7 @@ int bts_conv_set_producer_groups(int groups);
 int bts_wgrad2_set_tma(int on);
 int bts_wgrad2_set_min_pixels(long long n);
 int bts_wgrad2_set_min_kblocks(int n);
-int bts_wgrad2_set_pointwise(int on);        /* 1 (default): 1x1 layers with 64 < Cout <= 256 use this kernel too */       /* fewest 16-pixel k-blocks per split-K CTA (default 8; n < 1 restores) */
+int bts_wgrad2_set_pointwise(int on);        /* 1 (default): 1x1 layers with 64 < Cout <= 256 use this kernel too */
 
 /* dgrad (or any act-free conv) whose epilogue also reduces the BatchNorm(+ReLU)-backward sums of the layer in front of the
  * conv: the tile written is g = dL/d[relu](bn(x_bn)); S1[c] += sum_p g*mask, S2[c] += sum_p g*mask*xhat (zero them first),
@@ -168,6 +166,8 @@ int bts_bn_bwd_coef(const double *S1, const double *S2, long long M, int C, cons
 /* grouped 3x3 (ResNeXt: 32 groups of cpg channels): w is (width, cpg, KH, KW).  bts_conv_group_window -> the diagonal block
  * width kwin the packed operator uses (128 when width % 128 == 0 and 128 % cpg == 0; 0 = not supported). */
 int bts_conv_group_window(int width, int cpg);
+/* n-tile width of the grouped operator of window kwin (the widest multiple of 16 <= 64 dividing kwin; 0 if kwin is invalid) */
+int bts_conv_group_n_tile(int kwin);
 long long bts_conv_packed_floats_grouped(int width, int cpg, int KH, int KW);
 int bts_conv_pack_weights_grouped(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw, int width,
                                   int cpg, int KH, int KW, int transpose_flip, int flags, float *wpack, void *stream);
@@ -178,7 +178,8 @@ int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, int B, int 
                            int splitK, float *dw, long long s_co, long long s_ci, long long s_kh, long long s_kw,
                            int precision, void *stream);
 
-/* wgrad on the same engine: dW[co,ci,tap] = sum_p dY[p,co] * pre(x[p (+) tap, ci]), MN-major tcgen05 operands,
+/* wgrad on the same engine: dW[co,ci,tap] = sum_p dY[p,co] * pre(x[p (+) tap, ci]), both operands transposed
+ * to K-major in shared memory,
  * split-K partials in `workspace` reduced deterministically into dw (strides in floats).
  *   bts_conv_wgrad_plan(...) -> splitK and the workspace size (floats) the call needs. */
 int bts_conv_wgrad_plan(int B, int Hout, int Wout, int Cin, int Cout, int KH, int KW, int stride, int *splitK_out,

@@ -1,6 +1,6 @@
 // TensorFlow custom-op registration shim over the bts_b200 C ABI (SURVEY 8f rank 4, "TF-op surface").
 //
-// Re-exposes the sm_100a LPG kernels behind the op names / signatures the reference's TF graph code binds:
+// Re-exposes the sm_90a LPG kernels behind the op names / signatures the reference's TF graph code binds:
 //   lpg.local_planar_guidance(plane_eq, upratio=r, focal=...)        tensorflow/bts.py:279,294,309
 //   lpg.local_planar_guidance_grad(depth_grad, input, focal)         tensorflow/custom_layer/_local_planar_guidance_grad.py:33
 // i.e. ops "LocalPlanarGuidance" (input: float[B,h,w,4], focal: float[B], attr upratio:int -> depth: float[B,h*r,w*r]) and

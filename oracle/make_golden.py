@@ -18,6 +18,27 @@ from ref_shim import load_reference  # noqa: E402
 OUT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests", "golden")
 
 
+PART_BYTES = 900 * 1024      # fixture files stay below 1 MB: larger sets are split into NAME.npz + NAME.partK.npz
+
+
+def save_split(name, d):
+    """np.savez_compressed of d as NAME.npz, spilling arrays into NAME.part1.npz, ... (tests/conftest.py merges them).
+    Part files of an earlier, larger set are removed first so that the loader never merges stale arrays."""
+    import glob
+    for old in glob.glob(os.path.join(OUT, name + ".part*.npz")):
+        os.remove(old)
+    parts, cur, size = [], {}, 0
+    for k, v in d.items():
+        if cur and size + v.nbytes > PART_BYTES:
+            parts.append(cur)
+            cur, size = {}, 0
+        cur[k] = v
+        size += v.nbytes
+    parts.append(cur)
+    for i, part in enumerate(parts):
+        np.savez_compressed(os.path.join(OUT, name + (".part%d" % i if i else "") + ".npz"), **part)
+
+
 def head_planes(B, h, w, max_depth, gen):
     """Plane coefficients through the real head parametrisation (BASELINE.md LPG-u inputs)."""
     z = torch.randn(B, 3, h, w, generator=gen)
@@ -27,10 +48,98 @@ def head_planes(B, h, w, max_depth, gen):
     return torch.stack([torch.sin(th) * torch.cos(ph), torch.sin(th) * torch.sin(ph), torch.cos(th), d], 1).contiguous()
 
 
+# cases of tests/test_io_oracle.py: the inputs are regenerated there from the same seeds, only the reference's answers are stored
+IO_DATASETS = ("nyu", "kitti")
+IO_SEEDS = 6
+# (B, h, w, r, seed) of tests/test_oracle_properties.py: drawn once from its hypothesis strategy's ranges
+LPG_SHAPES = [(1, 1, 1, 2, 0), (1, 6, 7, 8, 1), (3, 1, 7, 4, 2), (2, 5, 3, 2, 3), (3, 6, 1, 8, 4), (1, 3, 4, 4, 5),
+              (2, 2, 6, 8, 6), (3, 4, 5, 2, 999983), (2, 6, 7, 4, 123456), (1, 5, 2, 8, 777), (3, 3, 3, 2, 42), (2, 1, 4, 4, 10 ** 6)]
+# encoders of tests/test_oracle.py::test_oracle_model_vs_live_reference_full_model
+FULL_MODELS = ("densenet121_bts", "resnext50_bts", "mobilenetv2_bts")
+
+
+def io_reference(R):
+    """The reference's compute_errors (bts_main.py, extracted by ast: the script parses argv at import) and its training
+    transform (bts_dataloader.py random_crop / train_preprocess / ToTensor) on the seeded inputs of test_io_oracle.py."""
+    import ast
+    import random
+    from ref_shim import REFERENCE_DIR
+    d = {}
+    src = open(os.path.join(REFERENCE_DIR, "bts_main.py")).read()
+    fn = [n for n in ast.parse(src).body if isinstance(n, ast.FunctionDef) and n.name == "compute_errors"][0]
+    ns = {"np": np}
+    exec(compile(ast.Module([fn], []), "bts_main.compute_errors", "exec"), ns)
+    rng = np.random.RandomState(0)
+    gt = rng.uniform(0.5, 70, 5000).astype(np.float32)
+    pred = (gt * rng.uniform(0.6, 1.6, 5000)).astype(np.float32)
+    d["compute_errors"] = np.array(ns["compute_errors"](gt, pred), dtype=np.float64)
+    sys.path.insert(0, REFERENCE_DIR)
+    import importlib
+    D = importlib.import_module("bts_dataloader")
+    for dataset in IO_DATASETS:
+        ds = D.DataLoadPreprocess.__new__(D.DataLoadPreprocess)
+        ds.args = types.SimpleNamespace(dataset=dataset)
+        rng = np.random.RandomState(1)
+        img_u8 = rng.randint(0, 256, (40, 56, 3)).astype(np.uint8)
+        dep_u16 = rng.randint(0, 60000, (40, 56)).astype(np.uint16)
+        div = 1000.0 if dataset == "nyu" else 256.0
+        for seed in range(IO_SEEDS):
+            random.seed(seed)
+            np.random.seed(seed)
+            image = np.asarray(img_u8, dtype=np.float32) / 255.0
+            depth = np.expand_dims(np.asarray(dep_u16, dtype=np.float32), 2) / div
+            ci, cd = ds.random_crop(image, depth, 32, 32)
+            ri, rd = ds.train_preprocess(ci, cd)
+            sample = D.ToTensor("train")({"image": ri, "depth": rd, "focal": 1.0})
+            d["%s_%d_image" % (dataset, seed)] = sample["image"].numpy()
+            d["%s_%d_depth" % (dataset, seed)] = sample["depth"].numpy()
+    np.savez_compressed(os.path.join(OUT, "io_reference.npz"), **d)
+
+
+def lpg_shapes(R):
+    """local_planar_guidance of the reference on the planes tests/conftest.py:head_planes draws for LPG_SHAPES."""
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "tests"))
+    from conftest import head_planes as planes
+    d = {"shapes": np.array(LPG_SHAPES, dtype=np.int64)}
+    for i, (B, h, w, r, seed) in enumerate(LPG_SHAPES):
+        plane = planes(B, h, w, 10.0, seed=seed)
+        want = R.local_planar_guidance(r)(plane, torch.full((B,), 518.8579))
+        d["depth%d" % i] = (want.squeeze(1) if want.dim() == 4 else want).numpy()
+    np.savez_compressed(os.path.join(OUT, "lpg_shapes.npz"), **d)
+
+
+def full_models(R):
+    """The reference BtsModel with the weights the oracle model draws under torch.manual_seed(0) (so that the test can
+    rebuild them without the reference), eval and train mode, on the seeded inputs of test_oracle.py."""
+    import bts_oracle as O
+    d = {}
+    for enc in FULL_MODELS:
+        p = types.SimpleNamespace(encoder=enc, max_depth=10.0, dataset="nyu", bts_size=512)
+        torch.manual_seed(0)
+        orc = O.OracleModel(enc, 10.0, "nyu", 512)
+        ref = R.BtsModel(p)
+        ref.load_state_dict(orc.state_dict(), strict=True)
+        x = torch.randn(1, 3, 64, 96, generator=torch.Generator().manual_seed(1))
+        focal = torch.tensor([518.8579])
+        for mode in ("eval", "train"):
+            getattr(ref, mode)()
+            if mode == "train":
+                x = torch.cat([x, x.flip(3)], 0)
+                focal = torch.tensor([518.8579, 518.8579])
+            with torch.no_grad():
+                outs = ref(x, focal)
+            d.update({"%s_%s_out%d" % (enc, mode, i): o.numpy() for i, o in enumerate(outs)})
+    np.savez_compressed(os.path.join(OUT, "full_models.npz"), **d)
+
+
 def main():
     os.makedirs(OUT, exist_ok=True)
     R = load_reference()
     torch.set_num_threads(4)
+    if len(sys.argv) > 1:                  # named fixture sets only, e.g. `make_golden.py io_reference full_models`
+        for name in sys.argv[1:]:
+            globals()[name](R)
+        return
 
     # ---- LPG: forward + autograd gradient, r = 2, 4, 8 (pytorch/bts.py:124-146)
     for r in (2, 4, 8):
@@ -97,7 +206,10 @@ def main():
             outs = dec(feats, focal)
         d.update({"train_out%d" % i: o.numpy() for i, o in enumerate(outs)})
         d.update({"sd_after." + k: v.numpy() for k, v in dec.state_dict().items() if "running" in k})
-        np.savez_compressed(os.path.join(OUT, "decoder_%s.npz" % dataset), **d)
+        save_split("decoder_%s" % dataset, d)
+    io_reference(R)
+    lpg_shapes(R)
+    full_models(R)
     print("golden fixtures written to", os.path.abspath(OUT))
     for f in sorted(os.listdir(OUT)):
         print("  %-24s %8d bytes" % (f, os.path.getsize(os.path.join(OUT, f))))

@@ -17,7 +17,7 @@ os.environ.setdefault("BTS_B200_PRETRAINED", "0")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -31,8 +31,13 @@ def pytest_collection_modifyitems(config, items):
 
 @pytest.fixture(scope="session")
 def golden():
-    def load(name):
-        return dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+    def load(name):          # NAME.npz plus its NAME.partK.npz spill files (oracle/make_golden.py keeps each below 1 MB)
+        d = dict(np.load(os.path.join(GOLDEN, name + ".npz")))
+        k = 1
+        while os.path.isfile(os.path.join(GOLDEN, "%s.part%d.npz" % (name, k))):
+            d.update(np.load(os.path.join(GOLDEN, "%s.part%d.npz" % (name, k))))
+            k += 1
+        return d
     return load
 
 

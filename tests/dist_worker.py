@@ -53,7 +53,7 @@ def main():
         worst = max(worst, err)
         errs.append(err)
         assert err < 1e-5, "%s: DDP gradient differs from the mean of the per-shard gradients by %.3g" % (k, err)
-    # (1b) the B200-native schedule of bench.py -- bts_b200.dist.FlatGradReducer -- produces the same averaged gradients
+    # (1b) the native schedule of bench.py -- bts_b200.dist.FlatGradReducer -- produces the same averaged gradients
     from bts_b200 import dist as D
     flat_m = build()
     red = D.FlatGradReducer(flat_m.parameters())

@@ -27,7 +27,7 @@ def test_library_builds_and_exports_every_declared_symbol():
         assert hasattr(L, s), "libbts_b200.so does not export %s" % s
     assert sorted(_lib.SIGNATURES) == syms          # ctypes table covers exactly the header
     buf = ctypes.create_string_buffer(128)
-    assert L.bts_version(buf, 128) == 100 and b"sm_100a" in buf.value
+    assert L.bts_version(buf, 128) == 90 and b"sm_90a" in buf.value
 
 
 def test_ops_refuse_cpu_tensors_no_fallback():

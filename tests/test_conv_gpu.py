@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 implicit-GEMM conv engine through the C-ABI.
+"""GPU parity tests of the wgmma implicit-GEMM conv engine through the C-ABI.
 Checker: torch fp64 conv2d on the CPU (the engine is a floating-point kernel; tolerance stated per test:
 3xTF32 parity mode must match fp32-grade, <= 2e-5 of the output scale; the reference's own fp32 noise is ~1e-6)."""
 import pytest

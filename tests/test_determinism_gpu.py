@@ -1,7 +1,6 @@
 """A training step of the engine is bit-reproducible run to run: every reduction either has a fixed order (warp butterflies,
-per-warp shared-memory partials, split-K partial buffers summed by a second kernel) or is accumulated in fp64.  (Round 2: the
-fp32 shared-memory atomics of the conv-epilogue BatchNorm statistics used to make two identical steps differ by 3e-3 of the
-gradient -- tools/determinism_probe.py, profiles/r02_determinism_{before,after}.txt.)"""
+per-warp shared-memory partials, split-K partial buffers summed by a second kernel) or is accumulated in fp64
+(tools/determinism_probe.py reports the worst difference between two identical steps)."""
 import types
 
 import pytest

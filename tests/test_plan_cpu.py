@@ -1,11 +1,11 @@
 """Host-side planning logic of the conv engine through the C ABI (no GPU, no kernel launches): split-K plans and workspace
 sizes of the wgrad kernels on the K16 layer shapes, routing switches, operator-packing sizes, eligibility tables.
-Without a device the library plans for 148 SMs (B200)."""
+Without a device the library plans for 132 SMs (H100 SXM)."""
 import ctypes
 
 import pytest
 
-SMS = 148
+SMS = 132
 
 # (B, H, W, Cin, Cout, K) of DenseNet-161 / decoder layers at the K16 config
 LAYERS = [(16, 88, 176, 192, 48, 3), (16, 44, 88, 192, 48, 3), (16, 22, 44, 192, 48, 3), (16, 11, 22, 192, 48, 3),
@@ -42,9 +42,11 @@ def test_wgrad_plan_workspace_and_wave_fill(layer):
 
 def test_narrow_output_routing_fills_one_wave_and_respects_the_switches():
     L = _lib()
-    # dense 3x3 192->48 @22x44x16 = 15488 pixels: shifted-dY kernel, 2 channel tiles x split-K = one full wave of 148 CTAs
+    # dense 3x3 192->48 @22x44x16 = 15488 pixels: shifted-dY kernel, 3 input-channel tiles x 3 output-channel groups x
+    # split-K CTAs fill whole waves of the SMs
     split, _ = _plan(L, 16, 22, 44, 192, 48, 3)
-    assert 2 * split == SMS
+    ctas = 9 * split
+    assert ctas / (-(-ctas // SMS) * SMS) >= 0.98
     # every CTA keeps at least min_kblocks k-blocks of 16 pixels
     assert (15488 // 16) // split >= 8
     L.bts_wgrad2_set_min_kblocks(64)

@@ -1,5 +1,5 @@
 """GPU parity tests of the ResNet / ResNeXt encoder pieces (reference pytorch/bts.py:282-296 via torchvision.models.resnet):
-grouped 3x3 convolution as a block-diagonal tcgen05 operator (forward, dgrad, wgrad), the dgrad of stride-2 convolutions
+grouped 3x3 convolution as a block-diagonal tensor-core operator (forward, dgrad, wgrad), the dgrad of stride-2 convolutions
 (zero-stuffed source), the stem max-pool and the bottleneck tail relu(bn(x) + identity).
 Checker: torch fp64 on the CPU; tolerance 2e-5 of the output scale (fp32-grade, as tests/test_conv_gpu.py)."""
 import pytest

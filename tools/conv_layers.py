@@ -1,4 +1,4 @@
-"""Per-layer timing of the tcgen05 conv engine vs cuDNN fp32 on K16 (B=16, 352x704) DenseNet-161 + decoder shapes.
+"""Per-layer timing of the wgmma conv engine vs cuDNN fp32 on K16 (B=16, 352x704) DenseNet-161 + decoder shapes.
 usage: python tools/conv_layers.py [fwd|dgrad|wgrad|all]"""
 import os, sys, time
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

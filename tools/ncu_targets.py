@@ -1,4 +1,4 @@
-"""One representative launch of each round-2 kernel family, for `ncu --set full` (see profiles/README.md).
+"""One representative launch of each kernel family, for `ncu --set full` where Nsight Compute is available.
 usage: ncu_targets.py conv_db1 | dgrad_db1 | dgrad_pw | fwd_pw | wgrad2_db1 | wgrad2_pw | bn_onepass   [iters]
 Shapes are the K16 ones (batch 16, DenseNet-161 block 1 / 2)."""
 import os
