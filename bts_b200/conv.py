@@ -66,8 +66,6 @@ def trace_report():
 if _os.environ.get("BTS_B200_TMA") is not None:            # bring-up switch for the TMA-staged activation tiles
     _lib.lib().bts_conv_set_tma(int(_os.environ["BTS_B200_TMA"]))
 
-if _os.environ.get("BTS_B200_GROUPS") is not None:         # activation-producer groups of the conv engine: 0 auto, 2, 4
-    _lib.lib().bts_conv_set_producer_groups(int(_os.environ["BTS_B200_GROUPS"]))
 if _os.environ.get("BTS_B200_W2_TMA") is not None:         # 0: narrow-output wgrad producers load from global memory
     _lib.lib().bts_wgrad2_set_tma(int(_os.environ["BTS_B200_W2_TMA"]))
 

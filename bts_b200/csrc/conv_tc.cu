@@ -13,23 +13,27 @@
 // GEMM view: M = B*Hout*Wout pixels (128 per CTA tile: two warpgroups of 64 rows), N = Cout (<= 64 per tile: the
 // k-block accumulator and the tile sum of a 64 x 64 tile are 64 registers per thread), K = the dense sequence of 16-byte channel quads,
 // tap-major, in blocks of 32 fp32 (one 128-byte swizzled row per pixel).
-// Precision: fp32 operands are split x = hi + lo with hi = rna_tf32(x), lo = rna_tf32(x - hi) and the tile
-// accumulates  A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with tf32 wgmma into fp32 register accumulators (error
-// ~2^-21 per product: fp32-grade, SURVEY Appendix F); every k-block's tensor-core sum is added into the tile sum with
-// round-to-nearest fp32 adds.
+// Precision: fp32 operands are split x = hi + lo with hi = x rounded to tf32, lo = x - hi and the tile accumulates
+// A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with tf32 wgmma into fp32 register accumulators (error ~2^-21 per product:
+// fp32-grade, SURVEY Appendix F); every k-block's tensor-core sum is added into the tile sum with round-to-nearest fp32
+// adds.  The weights are split once, when they are packed; the activations are split by the consumers in registers.
 // Single-pass TF32 is available as an explicitly labelled fast mode (precision=1) and is NOT used for parity.
 //
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... with the smem stage
-// ring and all warp roles running continuously across tile boundaries (the loader and producers fill the stages of tile
-// t+1 while the consumers run the epilogue of tile t; no per-tile launch or pipeline-fill cost).
-// Warp roles (288 + 128 G threads, 1 CTA/SM):
-//   warps 0..7  : two consumer warpgroups -- wgmma on the staged operands, then the epilogue from the accumulator
-//                 registers: activation, NHWC stores, optional BatchNorm batch statistics of the output;
-//   warp 8      : weight loader -- one thread streams pre-packed, pre-split, pre-swizzled weight tiles with 1-D bulk
-//                 async copies (cp.async.bulk) completing on an mbarrier (and, in TMA mode, the im2col activation tile);
-//   warps 9..   : G producer groups (alternating k-blocks): coalesced 128-bit global loads of the activation
-//                 tile (8 lanes cover one pixel's 128 B), pre-op + hi/lo split in registers, swizzled 128-bit
-//                 shared stores of both halves, fence.proxy.async, mbarrier arrive.
+// ring and all warp roles running continuously across tile boundaries (the producers fill the stages of tile t+1 while
+// the consumers run the epilogue of tile t; no per-tile launch or pipeline-fill cost).
+// Warp roles (512 threads = 16 warps, 128 registers per thread, 1 CTA/SM):
+//   warps 0..7  : two consumer warpgroups -- per k-block, each thread loads its A fragments (fp32) from the swizzled tile,
+//                 splits them into hi/lo in registers and issues register-A wgmma against the B hi/lo tiles in shared
+//                 memory; then the epilogue from the accumulator registers: activation, NHWC stores, optional BatchNorm
+//                 batch statistics of the output;
+//   warps 8..15 : two producer groups (alternating k-blocks).  One lane of the group filling a k-block streams its
+//                 pre-packed, pre-split, pre-swizzled weight tile with a 1-D bulk async copy (cp.async.bulk) completing on
+//                 the stage's mbarrier (in TMA mode also the im2col activation tile); the group's threads make coalesced
+//                 128-bit global loads of the activation tile (8 lanes cover one pixel's 128 B), apply the pre-op in
+//                 registers, one swizzled 128-bit shared store per (row, chunk), fence.proxy.async, mbarrier arrive.
+// Staging A as fp32 and splitting it in the consumers keeps shared-memory traffic per k-block at one A tile written and
+// read once (A from shared memory through descriptors would be read by each of the three products).
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -44,11 +48,10 @@ namespace {
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 32;                 // fp32 elements per k-block = one 128-byte row
 constexpr int MAX_N = 64;                   // output channels per tile (two register accumulators per consumer thread)
-constexpr int A_TILE_BYTES = BLOCK_M * 128; // 16 KB (hi or lo)
+constexpr int A_TILE_BYTES = BLOCK_M * 128; // 16 KB of fp32 activations
 constexpr int CONSUMER_THREADS = 256;       // two warpgroups
-constexpr int LOADER_WARP = CONSUMER_THREADS / 32;
 constexpr int PRODUCER_THREADS = 128;       // per group
-constexpr int FOUR_GROUPS_MAX_N = 48;       // widest tile run with four producer groups
+constexpr int NUM_THREADS = CONSUMER_THREADS + 2 * PRODUCER_THREADS;   // 16 warps: 128 registers per thread
 constexpr int MAX_CIN_SMEM = 4096;          // pre-op scale/shift staged in smem (32 KB at most)
 
 struct ConvParams {
@@ -90,7 +93,7 @@ struct ConvParams {
     const float *bnb_x; long long bnb_xs;
     const float *bnb_st;             // [4][Cout]: scale, shift, mean, invstd
     int bnb_relu;
-    int stages, stage_bytes; // smem ring: as many (A hi/lo + B hi/lo) stages as fit
+    int stages, stage_bytes; // smem ring: as many (A + B hi/lo) stages as fit
     tc::FastDiv fd_wout, fd_hout, fd_ntiles;
 };
 
@@ -197,7 +200,7 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackDesc 
 
 // ------------------------------------------------------------------------------------------- main kernel
 // dynamic smem, 1024-byte aligned base:
-//   [S stages][A_hi 16K | A_lo 16K | B_hi n_tile*128 | B_lo n_tile*128]   S = as many stages as fit (2..MAX_STAGES)
+//   [S stages][A 16K | B_hi n_tile*128 | B_lo n_tile*128]   S = as many stages as fit (2..MAX_STAGES)
 //   [pre-op scale[KC*32], shift[KC*32]]  (PRE >= 2 only)   [mbarriers]   [epilogue statistics partials]
 constexpr int MAX_STAGES = 6;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in maximum per CTA
@@ -212,17 +215,12 @@ constexpr int STAT_SETS = CONSUMER_THREADS / 32;
 // Index arithmetic: every k-block -> (tile, tap, channel chunk, stage, phase) mapping is carried in incrementally updated
 // counters, and the per-tile pixel decode uses multiply-shift division by host-precomputed constants (FastDiv).
 // TMA = true: the activation tile is staged by the Tensor Memory Accelerator (one cp.async.bulk.tensor im2col load per
-// k-block lands 128 pixels x 32 channels, swizzled, zero-filled where the filter tap falls into the padding) and is used
-// AS IS as the A_hi operand (the tensor core reads the top 19 bits of each fp32 word); the producer warps only derive
-// A_lo = x - trunc_tf32(x) from shared memory (and apply the BN/ReLU pre-op in place) -- no global loads, no address /
-// bounds arithmetic, one shared store instead of two.  K is enumerated per tap in 32-channel chunks (identical to the
-// dense-quad order whenever the K channels are a multiple of 32, which the host requires), stride 1, no up-sample.
-// G: producer groups (4 warps each).  G = 2 keeps one k-block of register prefetch per thread (two F4[8] buffers); G = 4
-// (narrow-N layers with >= 4 stages) drops the second buffer and lets the other groups' work hide a group's load latency.
-template <int PRE, int UP, bool VEC, bool TMA, int G>
-__global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_kernel(const ConvParams p,
-                                                                                      const __grid_constant__ CUtensorMap tmap) {
-    constexpr int NUM_THREADS = CONSUMER_THREADS + 32 + 128 * G;
+// k-block lands 128 pixels x 32 channels, swizzled, zero-filled where the filter tap falls into the padding) and IS the A
+// tile; the producer warps only apply the BN/ReLU pre-op in place (PRE != 0) -- no global loads, no address / bounds
+// arithmetic.  K is enumerated per tap in 32-channel chunks (identical to the dense-quad order whenever the K channels are
+// a multiple of 32, which the host requires), stride 1, no up-sample.
+template <int PRE, int UP, bool VEC, bool TMA>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-byte aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -233,12 +231,12 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + p.KC * 32;
     const uint32_t bar_off = pre_off + (PRE >= 2 ? (uint32_t)p.KC * 32u * 8u : 0u);
-    // bars: [0..MS) full (128 producer arrivals [+ the weight loader's expect_tx arrival and its bytes]), [MS..2MS) raw
-    // (TMA mode: the activation tile and the weights land there), [2MS..3MS) empty (one arrival per consumer warp)
+    // bars: [0..MS) full (the filling group's 128 producer arrivals [+ its expect_tx arrival for the weight bytes]),
+    // [MS..2MS) raw (TMA mode: the activation tile and the weights land there), [2MS..3MS) empty (one arrival per consumer
+    // warp)
     const uint32_t bar0 = base + bar_off;
-    auto full_a = [&](int s) { return bar0 + 8u * s; };
+    auto full = [&](int s) { return bar0 + 8u * s; };
     auto raw = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
-    auto full_b = [&](int s) { return TMA ? raw(s) : full_a(s); };
     auto empty = [&](int s) { return bar0 + 8u * (2 * MAX_STAGES + s); };
     double *s_stat = reinterpret_cast<double *>(sm + bar_off + BAR_BYTES);    // [8 warps][2][n_tile], only when p.stat_sum
 
@@ -249,11 +247,10 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
         for (int i = threadIdx.x; i < STAT_SETS * 2 * n_tile; i += NUM_THREADS) s_stat[i] = 0.0;
     // tiles of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...   (tile -> m_tile = tile / n_tiles, nt = tile % n_tiles)
     const int my_tiles = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-    const int total_kb = my_tiles * KB;          // host guarantees < 2^31
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
-            mbar_init(full_a(s), TMA ? PRODUCER_THREADS : PRODUCER_THREADS + 1);
+            mbar_init(full(s), TMA ? PRODUCER_THREADS : PRODUCER_THREADS + 1);
             mbar_init(raw(s), 1);
             mbar_init(empty(s), CONSUMER_THREADS / 32);
         }
@@ -267,50 +264,18 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
     }
     __syncthreads();
 
-    if (warp == LOADER_WARP) {
-        // ===================== weight loader =====================
-        if (lane == 0) {
-            const uint32_t bytes = 2u * (uint32_t)n_tile * 128u;
-            if (TMA) tma_prefetch_desc(&tmap);
-            int s = 0;
-            uint32_t ph = 0;
-            for (int ti = 0; ti < my_tiles; ++ti) {
-                const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-                const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
-                const int nt = tile - (int)m_tile * p.n_tiles;
-                const uint8_t *src = reinterpret_cast<const uint8_t *>(p.wpack) + (size_t)nt * KB * bytes;
-                const int win0 = p.kwin ? nt * n_tile / p.kwin * p.kwin : 0;     // grouped: first channel of the K window
-                int tw = 0, th = 0, tn = 0;
-                if (TMA) {                         // first output pixel of the tile -> base-pixel coordinate of the im2col walk
-                    const uint32_t m0 = m_tile * BLOCK_M;
-                    const uint32_t q = fdiv(m0, p.fd_wout);
-                    const uint32_t b = fdiv(q, p.fd_hout);
-                    tw = (int)(m0 - q * (uint32_t)p.Wout) - p.tma_adj;
-                    th = (int)(q - b * (uint32_t)p.Hout) - p.tma_adj;
-                    tn = (int)b;
-                }
-                int tap = 0, kc = 0;               // k-block -> (tap, chunk), advanced incrementally
-                for (int kb = 0; kb < KB; ++kb) {
-                    mbar_wait_sleep(empty(s), ph ^ 1);
-                    if (TMA) {
-                        mbar_arrive_expect_tx(raw(s), bytes + (uint32_t)A_TILE_BYTES);
-                        const int ky = (int)fdiv((uint32_t)tap, p.fd_kw), kx = tap - ky * p.KW;
-                        tma_im2col_4d(base + (uint32_t)s * stage_bytes, &tmap, win0 + kc * 32, tw, th, tn, raw(s),
-                                      (uint16_t)(kx * p.dil), (uint16_t)(ky * p.dil));
-                        if (++kc == p.KC) { kc = 0; ++tap; }
-                    } else {
-                        mbar_arrive_expect_tx(full_b(s), bytes);
-                    }
-                    bulk_copy_g2s(base + (uint32_t)s * stage_bytes + 2 * A_TILE_BYTES, src + (size_t)kb * bytes, bytes, full_b(s));
-                    if (++s == S) { s = 0; ph ^= 1; }
-                }
-            }
-        }
-    } else if (warp > LOADER_WARP) {
-        // ===================== activation producers (G groups x 4 warps) =====================
-        const int pt = threadIdx.x - (CONSUMER_THREADS + 32);
-        const int grp = pt >> 7;                   // producer group: global k-blocks gk == grp (mod G)
-        const int t = pt & 127;
+    if (threadIdx.x >= CONSUMER_THREADS) {
+        // ===================== producers (two groups x 4 warps, alternating k-blocks) =====================
+        // The group that fills a k-block also stages its weight tile: right after the stage has been released, one lane
+        // issues the 1-D bulk async copy (cp.async.bulk) of the pre-packed, pre-split, pre-swizzled B hi/lo rows -- and,
+        // in TMA mode, the im2col load of the activation tile -- completing on an mbarrier.
+        const int total_kb = my_tiles * KB;        // host guarantees < 2^31
+        const int pt = threadIdx.x - CONSUMER_THREADS;
+        const int grp = pt / PRODUCER_THREADS;     // producer group: global k-blocks gk == grp (mod 2)
+        const int t = pt % PRODUCER_THREADS;
+        const bool issuer = t == 0;
+        const uint32_t wbytes = 2u * (uint32_t)n_tile * 128u;
+        const uint8_t *wsrc = reinterpret_cast<const uint8_t *>(p.wpack);
         const int chunk = t & 7;                   // 16-byte chunk of the 128-byte row
         const int r0 = t >> 3;                     // rows r0 + 16*i, i = 0..7  (row & 7 == r0 & 7 for all of them)
         const int Hin = p.Hv, Win = p.Wv;
@@ -323,75 +288,95 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
         // swizzled byte offset of (row r0 + 16 i, chunk) inside a tile = roff0 + i * 2048
         const uint32_t roff0 = (uint32_t)r0 * 128u + (uint32_t)((chunk ^ (r0 & 7)) << 4);
         if constexpr (TMA) {
-            // ---- lo-producers: the raw tile is already in shared memory (TMA); derive A_lo (and the pre-op) in place
+            // ---- the raw tile lands in shared memory (TMA); apply the pre-op in place
             const bool need_mask = AFF && taps > 1;        // zero padding is applied AFTER the BatchNorm/ReLU pre-op
             int oyt[8], oxt[8];
             int ti = 0, kb = grp, cur = -1;
+            int nt = 0, win0 = 0, tw = 0, th = 0, tn = 0;
             while (kb >= KB) { kb -= KB; ++ti; }
             int s_t = grp;
             uint32_t ph_t = 0;
+            if (issuer) tma_prefetch_desc(&tmap);
             const int mine_t = (total_kb - grp + 1) >> 1;
             for (int it = 0; it < mine_t; ++it) {
-                int tap = 0, kc = kb;
-                if (taps > 1) { tap = (int)fdiv((uint32_t)kb, p.fd_kc); kc = kb - tap * p.KC; }
-                const int c = kc * 32 + chunk * 4;
-                uint32_t live = 0xffu;
-                if (need_mask) {
-                    if (ti != cur) {
-                        cur = ti;
-                        const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-                        const uint32_t m_base = fdiv((uint32_t)tile, p.fd_ntiles) * BLOCK_M + (uint32_t)r0;
+                if (ti != cur) {
+                    cur = ti;
+                    const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+                    const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
+                    nt = tile - (int)m_tile * p.n_tiles;
+                    win0 = p.kwin ? nt * n_tile / p.kwin * p.kwin : 0;     // grouped: first channel of the K window
+                    // first output pixel of the tile -> base-pixel coordinate of the im2col walk
+                    const uint32_t m0 = m_tile * BLOCK_M;
+                    const uint32_t q = fdiv(m0, p.fd_wout);
+                    const uint32_t b = fdiv(q, p.fd_hout);
+                    tw = (int)(m0 - q * (uint32_t)p.Wout) - p.tma_adj;
+                    th = (int)(q - b * (uint32_t)p.Hout) - p.tma_adj;
+                    tn = (int)b;
+                    if (need_mask) {
 #pragma unroll
                         for (int i = 0; i < 8; ++i) {
-                            const uint32_t m = m_base + 16u * i;
-                            const uint32_t q = fdiv(m, p.fd_wout);
-                            const uint32_t b = fdiv(q, p.fd_hout);
-                            oxt[i] = (int)(m - q * (uint32_t)p.Wout) - p.pad;
-                            oyt[i] = (int)(q - b * (uint32_t)p.Hout) - p.pad;
+                            const uint32_t m = m0 + (uint32_t)r0 + 16u * i;
+                            const uint32_t qi = fdiv(m, p.fd_wout);
+                            const uint32_t bi = fdiv(qi, p.fd_hout);
+                            oxt[i] = (int)(m - qi * (uint32_t)p.Wout) - p.pad;
+                            oyt[i] = (int)(qi - bi * (uint32_t)p.Hout) - p.pad;
                         }
                     }
-                    const int ky = (int)fdiv((uint32_t)tap, p.fd_kw), kx = tap - ky * KW;
-                    live = 0;
-#pragma unroll
-                    for (int i = 0; i < 8; ++i)
-                        live |= (((unsigned)(oyt[i] + ky * dil) < (unsigned)Hin && (unsigned)(oxt[i] + kx * dil) < (unsigned)Win) ? 1u : 0u) << i;
                 }
-                float sc[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
-                if (AFF) {
-                    const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
-                    const float4 b4 = *reinterpret_cast<const float4 *>(s_shift + c);
-                    sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
-                    sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
-                }
-                const uint32_t a_hi = base + (uint32_t)s_t * stage_bytes + roff0;
-                const uint32_t a_lo = a_hi + A_TILE_BYTES;
-                // First make sure the PREVIOUS use of this stage was consumed (what the loader waited for before re-arming
-                // raw): a parity wait only tells adjacent phases apart, and a group that runs ahead of the other group's
-                // k-block on the same stage would otherwise see the phase before last as "complete" and read a stale tile.
+                int tap = 0, kc = kb;
+                if (taps > 1) { tap = (int)fdiv((uint32_t)kb, p.fd_kc); kc = kb - tap * p.KC; }
+                const int ky = (int)fdiv((uint32_t)tap, p.fd_kw), kx = tap - ky * KW;
+                const uint32_t stage = base + (uint32_t)s_t * stage_bytes;
+                // The raw barrier is re-armed only after the stage's previous use was consumed: a parity wait only tells
+                // adjacent phases apart.
                 mbar_wait(empty(s_t), ph_t ^ 1);
-                mbar_wait(raw(s_t), ph_t);
-#pragma unroll
-                for (int i = 0; i < 8; ++i) {
-                    const float4 q4 = ld_shared_v4(a_hi + (uint32_t)i * 2048u);
-                    float v[4] = {q4.x, q4.y, q4.z, q4.w}, lo[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        float a = v[e];
-                        if (AFF) {
-                            a = fmaf(a, sc[e], sh[e]);              // scale/shift are 0 beyond Cin
-                            if (RELU) a = fmaxf(a, 0.f);
-                            a = ((live >> i) & 1u) ? a : 0.f;
-                        } else if (RELU) {
-                            a = fmaxf(a, 0.f);
-                        }
-                        v[e] = a;
-                        lo[e] = a - __uint_as_float(__float_as_uint(a) & 0xffffe000u);   // exact; hi = what the tensor core reads
-                    }
-                    if (PRE != 0) st_shared_v4(a_hi + (uint32_t)i * 2048u, v[0], v[1], v[2], v[3]);
-                    st_shared_v4(a_lo + (uint32_t)i * 2048u, lo[0], lo[1], lo[2], lo[3]);
+                if (issuer) {
+                    mbar_arrive_expect_tx(raw(s_t), wbytes + (uint32_t)A_TILE_BYTES);
+                    tma_im2col_4d(stage, &tmap, win0 + kc * 32, tw, th, tn, raw(s_t), (uint16_t)(kx * dil),
+                                  (uint16_t)(ky * dil));
+                    bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + ((size_t)nt * KB + kb) * wbytes, wbytes, raw(s_t));
                 }
-                fence_proxy_async();
-                mbar_arrive(full_a(s_t));
+                if constexpr (PRE != 0) {
+                    const int c = kc * 32 + chunk * 4;
+                    uint32_t live = 0xffu;
+                    if (need_mask) {
+                        live = 0;
+#pragma unroll
+                        for (int i = 0; i < 8; ++i)
+                            live |= (((unsigned)(oyt[i] + ky * dil) < (unsigned)Hin && (unsigned)(oxt[i] + kx * dil) < (unsigned)Win) ? 1u : 0u) << i;
+                    }
+                    float sc[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
+                    if (AFF) {
+                        const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
+                        const float4 b4 = *reinterpret_cast<const float4 *>(s_shift + c);
+                        sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
+                        sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
+                    }
+                    const uint32_t a_st = stage + roff0;
+                    mbar_wait(raw(s_t), ph_t);
+#pragma unroll
+                    for (int i = 0; i < 8; ++i) {
+                        const float4 q4 = ld_shared_v4(a_st + (uint32_t)i * 2048u);
+                        float v[4] = {q4.x, q4.y, q4.z, q4.w};
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            float a = v[e];
+                            if (AFF) {
+                                a = fmaf(a, sc[e], sh[e]);              // scale/shift are 0 beyond Cin
+                                if (RELU) a = fmaxf(a, 0.f);
+                                a = ((live >> i) & 1u) ? a : 0.f;
+                            } else if (RELU) {
+                                a = fmaxf(a, 0.f);
+                            }
+                            v[e] = a;
+                        }
+                        st_shared_v4(a_st + (uint32_t)i * 2048u, v[0], v[1], v[2], v[3]);
+                    }
+                    fence_proxy_async();
+                } else {
+                    mbar_wait(raw(s_t), ph_t);
+                }
+                mbar_arrive(full(s_t));
                 s_t += 2;
                 if (s_t >= S) { s_t -= S; ph_t ^= 1; }
                 kb += 2;
@@ -400,8 +385,10 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
         } else {
         // ---- LOAD cursor: (tile iteration, k-block in tile) of the next k-block this group loads; this lane's channel
         //      quad of that k-block is g = 8 kb + chunk -> (tap, quad in tap) by multiply-shift division
-        int oy[8], ox[8], rowoff[8];
-        int l_ti = 0, l_kb = grp, cur_ti = -1;      // (KB may be smaller than G)
+        // oyx[i]: the row's top-left source coordinate, (oy << 16) | (ox & 0xffff) -- one register per row instead of two,
+        // so that a k-block of loads in flight and one being stored fit the register budget (host: |coordinates| < 2^14)
+        int oyx[8], rowoff[8];
+        int l_ti = 0, l_kb = grp, cur_ti = -1, cur_nt = 0;      // (KB may be 1)
         while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
         auto set_tile = [&](int ti) {
             cur_ti = ti;
@@ -409,6 +396,7 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
             const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
             const uint32_t m_base = m_tile * BLOCK_M + (uint32_t)r0;
             const int nt = tile - (int)m_tile * p.n_tiles;
+            cur_nt = nt;
             const int cwin = p.kwin ? nt * p.n_tile / p.kwin * p.kwin : 0;     // first input channel of this n-tile's window
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -418,18 +406,20 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
                     const int x = (int)(m - q * (uint32_t)p.Wout);
                     const uint32_t b = fdiv(q, p.fd_hout);
                     const int y = (int)(q - b * (uint32_t)p.Hout);
-                    oy[i] = y * p.stride - p.pad;
-                    ox[i] = x * p.stride - p.pad;
-                    rowoff[i] = (int)b * p.Hs * Ws * xs + (UP ? 0 : (oy[i] * Ws + ox[i]) * xs) + cwin;
+                    const int oy = y * p.stride - p.pad, ox = x * p.stride - p.pad;
+                    oyx[i] = (int)(((uint32_t)oy << 16) | ((uint32_t)ox & 0xffffu));
+                    rowoff[i] = (int)b * p.Hs * Ws * xs + (UP ? 0 : (oy * Ws + ox) * xs) + cwin;
                 } else {
-                    oy[i] = ox[i] = -0x40000000;   // never in bounds
+                    oyx[i] = (int)0xc000c000u;     // (-0x4000, -0x4000): never in bounds
                     rowoff[i] = 0;
                 }
             }
         };
-        // ---- load phase: this lane's 8 x 16-byte global loads of one k-block (predicated, branch-free)
-        auto load_kb = [&](F4(&v)[8], uint32_t &mask, int &c_out) {
+        // ---- load phase: this lane's 8 x 16-byte global loads of one k-block (predicated, branch-free); w_out = index of
+        //      the k-block's weight tile in wpack (n-tile * KB + kb; host guarantees < 2^31)
+        auto load_kb = [&](F4(&v)[8], uint32_t &mask, int &c_out, int &w_out) {
             if (l_ti != cur_ti) set_tile(l_ti);
+            w_out = cur_nt * KB + l_kb;
             uint32_t g = (uint32_t)(l_kb * 8 + chunk);
             uint32_t tap = fdiv(g, p.fd_cq);
             if (p.chunk_major) {                   // (chunk, tap) order: one tap per k-block, the chunk advances every `taps` k-blocks
@@ -447,7 +437,7 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
             uint32_t mk = 0;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
-                const int yy = oy[i] + dy, xx = ox[i] + dx;
+                const int yy = (oyx[i] >> 16) + dy, xx = (int)(short)(oyx[i] & 0xffff) + dx;
                 bool ok = cok && (unsigned)yy < (unsigned)Hin && (unsigned)xx < (unsigned)Win;
                 if (UP == 2) ok = ok && (((yy | xx) & 1) == 0);          // zero-stuffed source: odd coordinates are zeros
                 mk |= (ok ? 1u : 0u) << i;
@@ -468,22 +458,23 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
                 }
             }
             mask = mk;
-            l_kb += G;
+            l_kb += 2;
             while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
         };
-        // ---- store phase: wait for the stage, pre-op + hi/lo split in registers, swizzled 128-bit stores, publish.
-        //      hi = fp32 rounded to tf32 (round-half-away on the 13 dropped bits, 2 integer ops); lo = x - hi is
-        //      exact in fp32 and the tensor core reads its top 19 bits (error <= 2^-21 |x|).
+        // ---- store phase: wait for the stage, stage its weights, pre-op in registers, swizzled 128-bit stores, publish
         int s_s = grp;                             // stage of this group's next store (S >= 2)
         uint32_t s_ph = 0;
-        while (s_s >= S) { s_s -= S; s_ph ^= 1; }
-        auto store_kb = [&](F4(&v)[8], uint32_t mask, const int c) {
-            const uint32_t a_hi = base + (uint32_t)s_s * stage_bytes + roff0;
-            const uint32_t a_lo = a_hi + A_TILE_BYTES;
-            const uint32_t bar_full = full_a(s_s);
+        auto store_kb = [&](F4(&v)[8], uint32_t mask, const int c, const int w) {
+            const uint32_t stage = base + (uint32_t)s_s * stage_bytes;
+            const uint32_t a_st = stage + roff0;
+            const uint32_t bar_full = full(s_s);
             mbar_wait(empty(s_s), s_ph ^ 1);
-            s_s += G;
-            while (s_s >= S) { s_s -= S; s_ph ^= 1; }
+            if (issuer) {
+                mbar_arrive_expect_tx(bar_full, wbytes);
+                bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + (size_t)w * wbytes, wbytes, bar_full);
+            }
+            s_s += 2;
+            if (s_s >= S) { s_s -= S; s_ph ^= 1; }
             float sc[4], sh[4];
             if (AFF) {
                 const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
@@ -499,116 +490,127 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
                     for (int e = 1; e < 4; ++e)
                         if (c + e >= Cin) v[i].v[e] = 0.f;
             }
-            // hi = fp32 rounded to tf32 (round-half-away on the 13 dropped bits, 2 integer ops); lo = x - hi is exact in fp32
-            // and the tensor core reads its top 19 bits.  (Truncating instead of rounding saves one op per element but
-            // makes lo one-signed: the dropped lo*lo term and lo's own truncation then add up coherently over K -- measured
-            // 2-3x the error, past the 2e-5 bar of tests/test_conv_gpu.py -- so the rounding stays.  A per-tile tap-mask +
-            // select-free interior path was also measured: more registers -> spills, fwd 27 -> 34 ms per K16 step.)
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
                 const bool live = (mask >> i) & 1u;
-                float hi[4], lo[4];
+                float a[4];
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
-                    float a = v[i].v[e];
+                    a[e] = v[i].v[e];
                     if (AFF) {
-                        a = fmaf(a, sc[e], sh[e]);              // scale/shift are 0 beyond Cin
-                        if (RELU) a = fmaxf(a, 0.f);
-                        a = live ? a : 0.f;                     // zero padding is applied after the pre-op
+                        a[e] = fmaf(a[e], sc[e], sh[e]);        // scale/shift are 0 beyond Cin
+                        if (RELU) a[e] = fmaxf(a[e], 0.f);
+                        a[e] = live ? a[e] : 0.f;               // zero padding is applied after the pre-op
                     } else if (RELU) {
-                        a = fmaxf(a, 0.f);                      // padded lanes were loaded as 0
+                        a[e] = fmaxf(a[e], 0.f);                // padded lanes were loaded as 0
                     }
-                    const float h = __uint_as_float((__float_as_uint(a) + 0x1000u) & 0xffffe000u);
-                    hi[e] = h;
-                    lo[e] = a - h;
                 }
-                st_shared_v4(a_hi + (uint32_t)i * 2048u, hi[0], hi[1], hi[2], hi[3]);
-                st_shared_v4(a_lo + (uint32_t)i * 2048u, lo[0], lo[1], lo[2], lo[3]);
+                st_shared_v4(a_st + (uint32_t)i * 2048u, a[0], a[1], a[2], a[3]);
             }
             fence_proxy_async();               // generic-proxy writes -> visible to the tensor-core (async) proxy
             mbar_arrive(bar_full);
         };
         // ---- software pipeline (register ping-pong): the loads of this group's next k-block -- possibly of the next
         //      tile -- are in flight while the current one is transformed and stored
-        const int mine = total_kb > grp ? (total_kb - grp + G - 1) / G : 0;   // k-blocks of this group
-        if constexpr (G == 2) {
-            F4 va[8], vb[8];
-            uint32_t ma = 0, mb = 0;
-            int ca = 0, cb = 0;
-            int issued = 0;
-            if (issued < mine) { load_kb(va, ma, ca); ++issued; }
-            for (int done = 0; done < mine; done += 2) {
-                if (issued < mine) { load_kb(vb, mb, cb); ++issued; }
-                store_kb(va, ma, ca);
-                if (done + 1 < mine) {
-                    if (issued < mine) { load_kb(va, ma, ca); ++issued; }
-                    store_kb(vb, mb, cb);
-                }
-            }
-        } else {
-            F4 va[8];
-            uint32_t ma = 0;
-            int ca = 0;
-            for (int done = 0; done < mine; ++done) {
-                load_kb(va, ma, ca);
-                store_kb(va, ma, ca);
+        const int mine = total_kb > grp ? (total_kb - grp + 1) / 2 : 0;   // k-blocks of this group
+        F4 va[8], vb[8];
+        uint32_t ma = 0, mb = 0;
+        int ca = 0, cb = 0, wa = 0, wb = 0;
+        int issued = 0;
+        if (issued < mine) { load_kb(va, ma, ca, wa); ++issued; }
+        for (int done = 0; done < mine; done += 2) {
+            if (issued < mine) { load_kb(vb, mb, cb, wb); ++issued; }
+            store_kb(va, ma, ca, wa);
+            if (done + 1 < mine) {
+                if (issued < mine) { load_kb(va, ma, ca, wa); ++issued; }
+                store_kb(vb, mb, cb, wb);
             }
         }
         }   // !TMA
     } else {
         // ===================== consumers: two warpgroups, rows [64 wg, 64 wg + 64) of every 128-pixel tile =========
-        // 3xTF32: per k8 step A_lo*B_hi, A_hi*B_lo, A_hi*B_hi (small cross terms first).  The tensor cores accumulate one
-        // k-block (4 k8 steps x 3 products) into `acc`; it is then added into the fp32 tile sum `tot` with round-to-nearest
-        // adds, which keeps the accumulation error of long-K layers at the level of a plain fp32 sum.  The stage is handed
-        // back to the loader / producers as soon as its wgmma group has completed.
+        // 3xTF32: every thread loads its A fragments of the k-block from the swizzled fp32 tile and splits them in
+        // registers: hi = x rounded to tf32 (round-half-away on the 13 dropped bits, 2 integer ops), lo = x - hi, exact in
+        // fp32 (the tensor core reads its top 19 bits: error <= 2^-21 |x|).  (Truncating instead of rounding saves one op
+        // but makes lo one-signed: the dropped lo*lo term and lo's own truncation then add up coherently over K -- measured
+        // 2-3x the error, past the 2e-5 bar of tests/test_conv_gpu.py -- so the rounding stays.)
+        // Per k8 step A_lo*B_hi, A_hi*B_lo, A_hi*B_hi (small cross terms first), A from registers, B from shared memory.
+        // The tensor cores accumulate one k-block (4 k8 steps x 3 products) into `acc`; it is then added into the fp32
+        // tile sum `tot` with round-to-nearest adds, which keeps the accumulation error of long-K layers at the level of a
+        // plain fp32 sum.  The stage is handed back to the producers as soon as its wgmma group has completed.
         const int wg = warp >> 2;
         const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // rows row and row + 8 of the tile
-        const int cq = (lane & 3) * 2;                               // columns 8 j + cq, 8 j + cq + 1
         const bool ovec = ((p.os & 1) == 0) && ((((uintptr_t)p.out) & 7) == 0);
         const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             constexpr int R = N / 2;
             float acc[R], tot[R];
-            const uint64_t dA0 = make_desc(base + (uint32_t)wg * (64u * 128u));      // A_hi of stage 0, this warpgroup's rows
-            const uint64_t oAlo = (uint64_t)(A_TILE_BYTES >> 4);
-            const uint64_t oBhi = (uint64_t)((2 * A_TILE_BYTES - wg * 64 * 128) >> 4);
-            const uint64_t oBlo = oBhi + (uint64_t)((N * 128) >> 4), stage_step = (uint64_t)(stage_bytes >> 4);
+            // A fragment of k8 step k (wgmma_tf32.cuh): (row, 8k + q), (row + 8, 8k + q), (row, 8k + q + 4),
+            // (row + 8, 8k + q + 4) with q = lane % 4.  16-byte chunk c of a row sits at chunk c ^ (row & 7) of its
+            // 128-byte line (SWIZZLE_128B), the same for row + 8; the chunk bits of aF hold row & 7, so the address of
+            // chunk c is aF ^ (c << 4)
+            const uint32_t aF0 = base + (uint32_t)row * 128u + ((uint32_t)(row & 7) << 4) + (threadIdx.x & 3u) * 4u;
+            const uint64_t dB0 = make_desc(base + A_TILE_BYTES);                              // B_hi of stage 0
+            const uint64_t oBlo = (uint64_t)((N * 128) >> 4), stage_step = (uint64_t)(stage_bytes >> 4);
             int s = 0;
             uint32_t ph = 0;
-            uint64_t d = dA0;
+            uint32_t aF = aF0;
+            uint64_t d = dB0;
             for (int ti = 0; ti < my_tiles; ++ti) {
                 const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
                 const int m_tile = (int)fdiv((uint32_t)tile, p.fd_ntiles), nt = tile - m_tile * p.n_tiles;
 #pragma unroll
                 for (int i = 0; i < R; ++i) tot[i] = 0.f;
                 for (int kb = 0; kb < KB; ++kb) {
-                    mbar_wait(full_a(s), ph);
-                    wgmma_fence();
-                    const uint64_t dah = d, dal = d + oAlo, dbh = d + oBhi, dbl = d + oBlo;
+                    mbar_wait(full(s), ph);
+                    uint32_t hi[BLOCK_K / 8][4], lo[BLOCK_K / 8][4];
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / 8; ++k) {
-                        const uint32_t accumulate = k != 0;
-                        if (single) {
-                            Wgmma<N>::mma(acc, dah + 2 * k, dbh + 2 * k, accumulate);
-                        } else {
-                            Wgmma<N>::mma(acc, dal + 2 * k, dbh + 2 * k, accumulate);
-                            Wgmma<N>::mma(acc, dah + 2 * k, dbl + 2 * k, 1);
-                            Wgmma<N>::mma(acc, dah + 2 * k, dbh + 2 * k, 1);
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {                      // j: row + 8 (j & 1), column + 4 (j >> 1)
+                            const uint32_t x = ld_shared_u32((aF ^ (uint32_t)(32 * k + 16 * (j >> 1))) + 1024u * (j & 1));
+                            const uint32_t h = (x + 0x1000u) & 0xffffe000u;
+                            hi[k][j] = h;
+                            lo[k][j] = __float_as_uint(__uint_as_float(x) - __uint_as_float(h));
+                        }
+                    }
+                    wgmma_fence();
+                    if (single) {
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 8; ++k) Wgmma<N>::mma_rs(acc, hi[k], d + 2 * k, k != 0);
+                    } else {
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 8; ++k) {
+                            const uint64_t dbh = d + 2 * k, dbl = dbh + oBlo;
+                            Wgmma<N>::mma_rs(acc, lo[k], dbh, k != 0);
+                            Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
+                            Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
                         }
                     }
                     wgmma_commit();
                     wgmma_wait<0>();
                     wgmma_fence_operands(acc);
+#pragma unroll
+                    for (int k = 0; k < BLOCK_K / 8; ++k) {
+                        wgmma_fence_operands(hi[k]);
+                        wgmma_fence_operands(lo[k]);
+                    }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(empty(s));
 #pragma unroll
                     for (int i = 0; i < R; ++i) tot[i] += acc[i];
                     d += stage_step;
-                    if (++s == S) { s = 0; ph ^= 1; d = dA0; }
+                    aF += stage_bytes;
+                    if (++s == S) { s = 0; ph ^= 1; d = dB0; aF = aF0; }
                 }
 
-                // ---- epilogue straight from the accumulator registers
+                // ---- epilogue straight from the accumulator registers.  Its inputs are re-read per tile through an empty
+                //      asm: left loop-invariant, the per-column indices and addresses derived from them (dozens of values)
+                //      are computed before the tile loop and spill across the k-block loop.
+                int cq = ((int)threadIdx.x & 3) * 2, Cout = p.Cout;      // columns 8 j + cq, 8 j + cq + 1
+                const float *bnb_x = p.bnb_x, *bnb_st = p.bnb_st;
+                asm volatile("" : "+r"(cq), "+r"(Cout), "+l"(bnb_x), "+l"(bnb_st));
                 const long long m0 = (long long)m_tile * BLOCK_M + row, m1 = m0 + 8;
                 float *orow0 = p.out + (m0 < p.M ? m0 : 0) * p.os + (long long)nt * n_tile;
                 float *orow1 = p.out + (m1 < p.M ? m1 : 0) * p.os + (long long)nt * n_tile;
@@ -628,11 +630,11 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
                         }
                         if ((i ? m1 : m0) < p.M) {
                             float *orow = i ? orow1 : orow0;
-                            if (ovec && cabs + 1 < p.Cout) {
+                            if (ovec && cabs + 1 < Cout) {
                                 *reinterpret_cast<float2 *>(orow + col) = make_float2(o[0], o[1]);
                             } else {
-                                if (cabs < p.Cout) orow[col] = o[0];
-                                if (cabs + 1 < p.Cout) orow[col + 1] = o[1];
+                                if (cabs < Cout) orow[col] = o[0];
+                                if (cabs + 1 < Cout) orow[col + 1] = o[1];
                             }
                         }
                     }
@@ -653,12 +655,12 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
 #pragma unroll
                             for (int i = 0; i < 2; ++i) {
                                 const long long m = i ? m1 : m0;
-                                if (m < p.M && ch < p.Cout) {
+                                if (m < p.M && ch < Cout) {
                                     const float g = tot[4 * j + 2 * i + c];
-                                    if (p.bnb_x) {
-                                        const float xv = __ldg(p.bnb_x + m * p.bnb_xs + ch);
-                                        const float sc = __ldg(p.bnb_st + ch), sh = __ldg(p.bnb_st + p.Cout + ch);
-                                        const float mu = __ldg(p.bnb_st + 2 * p.Cout + ch), is = __ldg(p.bnb_st + 3 * p.Cout + ch);
+                                    if (bnb_x) {
+                                        const float xv = __ldg(bnb_x + m * p.bnb_xs + ch);
+                                        const float sc = __ldg(bnb_st + ch), sh = __ldg(bnb_st + Cout + ch);
+                                        const float mu = __ldg(bnb_st + 2 * Cout + ch), is = __ldg(bnb_st + 3 * Cout + ch);
                                         const float y = fmaf(xv, sc, sh);
                                         const float gm = (!p.bnb_relu || y > 0.f) ? g : 0.f;
                                         s1 += gm;
@@ -674,7 +676,7 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
                                 s1 += __shfl_xor_sync(0xffffffffu, s1, w);
                                 s2 += __shfl_xor_sync(0xffffffffu, s2, w);
                             }
-                            if (lane < 4 && ch < p.Cout) {                 // this (warp, lane) owns the slot: plain adds
+                            if (lane < 4 && ch < Cout) {                 // this (warp, lane) owns the slot: plain adds
                                 double *mine = s_stat + (size_t)warp * 2 * n_tile;
                                 mine[col + c] += (double)s1;
                                 mine[n_tile + col + c] += (double)s2;
@@ -708,9 +710,7 @@ __global__ void __launch_bounds__(CONSUMER_THREADS + 32 + 128 * G, 1) conv_tc_ke
             case 16: consume(std::integral_constant<int, 16>()); break;
             case 32: consume(std::integral_constant<int, 32>()); break;
             case 48: consume(std::integral_constant<int, 48>()); break;
-            default:
-                if constexpr (G == 2) consume(std::integral_constant<int, 64>());   // four groups run n_tile <= 48 only
-                break;
+            default: consume(std::integral_constant<int, 64>()); break;
         }
         if (p.stat_sum && p.n_tiles == 1) {
             asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");
@@ -821,7 +821,6 @@ extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, lon
 
 // ---- TMA tensor map of the NHWC activation tensor, im2col mode (cuTensorMapEncodeIm2col through the runtime's driver
 //      entry-point query: no link-time dependency on libcuda)
-static int g_producer_groups = 0;   // 0 / 4: four groups where the ring has >= 4 stages, 2: always two
 static int g_tma_mode = 0;      // 0 off, 1 on, 2 on with base-pixel coordinates NOT shifted by the lower corner, 3 on + strict
 
 typedef CUresult (*EncodeIm2colFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
@@ -865,11 +864,8 @@ extern "C" int bts_conv_set_tma(int mode) {
     return 0;
 }
 extern "C" int bts_conv_get_tma(void) { return g_tma_mode; }
-extern "C" int bts_conv_set_producer_groups(int g) {
-    if (g != 0 && g != 2 && g != 4) return BTS_EINVAL;
-    g_producer_groups = g;
-    return 0;
-}
+// the kernel has one producer layout, two groups of 4 warps: 0 (default) and 2 select it, anything else is refused
+extern "C" int bts_conv_set_producer_groups(int g) { return g == 0 || g == 2 ? 0 : BTS_EINVAL; }
 
 
 struct BnBwdArgs {
@@ -917,6 +913,10 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.Hout = p.up == 2 ? out_h : (Hin + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
     p.Wout = p.up == 2 ? out_w : (Win + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
     if (p.Hout < 1 || p.Wout < 1) return BTS_EINVAL;
+    // the producers keep a row's source coordinates as two 16-bit halves of one register
+    if (Hin >= 0x4000 || Win >= 0x4000 || p.Hout >= 0x4000 || p.Wout >= 0x4000 || pad >= 0x4000 ||
+        dil * (KH - 1) >= 0x4000 || dil * (KW - 1) >= 0x4000)
+        return BTS_EINVAL;
     p.M = (long long)B * p.Hout * p.Wout;
     p.KC = (p.Cin + 31) / 32;
     p.CQ = (p.Cin + 3) / 4;
@@ -932,8 +932,8 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     p.fd_ntiles = make_fastdiv((uint32_t)p.n_tiles);
     const int pre = (pre_scale ? 2 : 0) | (p.pre_relu ? 1 : 0);
-    // shared-memory plan: stage = A hi/lo (2 x 16 KB) + B hi/lo (2 x n_tile x 128 B); as many stages as fit
-    p.stage_bytes = 2 * A_TILE_BYTES + 2 * p.n_tile * 128;
+    // shared-memory plan: stage = A (16 KB) + B hi/lo (2 x n_tile x 128 B); as many stages as fit
+    p.stage_bytes = A_TILE_BYTES + 2 * p.n_tile * 128;
     const int pre_bytes = pre >= 2 ? p.KC * 32 * 8 : 0;
     const int stat_bytes = stat_sum ? STAT_SETS * 2 * p.n_tile * 8 : 0;
     p.stages = (SMEM_LIMIT - 1024 - BAR_BYTES - pre_bytes - stat_bytes) / p.stage_bytes;
@@ -966,25 +966,17 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
             return rc;                                   // forced: report why the map could not be built
         }
     }
-    // four producer groups on the narrow layers (n_tile <= 48), where producing the activation tile, not the tensor
-    // cores, sets the k-block time; the 800-thread CTA leaves no registers for a wider accumulator
-    const bool four = !use_tma && p.stages >= 4 && p.n_tile <= FOUR_GROUPS_MAX_N && g_producer_groups != 2;
-#define BTS_LAUNCH_G(PRE, UP, VEC, TMA, G)                                                                         \
+#define BTS_LAUNCH(PRE, UP, VEC, TMA)                                                                              \
     do {                                                                                                           \
         static bool attr_set_[BTS_MAX_DEVICES] = {};                                                               \
         bool &attr_set = attr_set_[bts_cur_device()];                                                              \
         if (!attr_set) {                                                                                           \
-            err = cudaFuncSetAttribute(conv_tc_kernel<PRE, UP, VEC, TMA, G>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+            err = cudaFuncSetAttribute(conv_tc_kernel<PRE, UP, VEC, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
                                        SMEM_LIMIT);                                                                \
             if (err != cudaSuccess) return (int)err;                                                               \
             attr_set = true;                                                                                       \
         }                                                                                                          \
-        conv_tc_kernel<PRE, UP, VEC, TMA, G><<<grid, CONSUMER_THREADS + 32 + 128 * G, smem, (cudaStream_t)stream>>>(p, tmap);         \
-    } while (0)
-#define BTS_LAUNCH(PRE, UP, VEC, TMA)                                                                              \
-    do {                                                                                                           \
-        if (four && VEC && !TMA) BTS_LAUNCH_G(PRE, UP, true, false, 4);                                            \
-        else BTS_LAUNCH_G(PRE, UP, VEC, TMA, 2);                                                                   \
+        conv_tc_kernel<PRE, UP, VEC, TMA><<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(p, tmap);                    \
     } while (0)
 #define BTS_DISPATCH_UV(PRE)                                  \
     do {                                                      \
@@ -1001,7 +993,6 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     }
 #undef BTS_DISPATCH_UV
 #undef BTS_LAUNCH
-#undef BTS_LAUNCH_G
     BTS_LAUNCH_CHECK();
     return 0;
 }

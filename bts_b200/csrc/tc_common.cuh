@@ -31,24 +31,6 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (++spins > 200000000u) __trap();   // watchdog: a protocol bug must fail loudly, not hang the box
     }
 }
-// same protocol, for waits that are expected to be long (the weight loader waiting for a free stage): back off between
-// polls so the spinning lane does not take issue slots from the producer warps.
-__device__ __forceinline__ void mbar_wait_sleep(uint32_t bar, uint32_t parity) {
-    uint32_t ok = 0;
-    uint32_t spins = 0;
-    while (true) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(ok)
-            : "r"(bar), "r"(parity)
-            : "memory");
-        if (ok) break;
-        __nanosleep(32);
-        if (++spins > 50000000u) __trap();
-    }
-}
 __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                  "l"(src), "r"(bytes), "r"(bar)
@@ -87,6 +69,13 @@ template <int R>
 __device__ __forceinline__ void wgmma_fence_operands(float (&d)[R]) {
 #pragma unroll
     for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+// same for A-fragment registers of the register-operand form: placed after the wait, it keeps them allocated (and
+// unchanged) until the wgmma group that reads them has completed
+template <int R>
+__device__ __forceinline__ void wgmma_fence_operands(uint32_t (&a)[R]) {
+#pragma unroll
+    for (int i = 0; i < R; ++i) asm volatile("" : "+r"(a[i])::"memory");
 }
 
 // K-major, 128-byte swizzle shared-memory matrix descriptor (sm_90 wgmma): start>>4 | LBO (unused, 1) | SBO = 1024 B
@@ -155,6 +144,11 @@ __device__ __forceinline__ void cp_async_wait_dyn(int pending) {   // wait until
 __device__ __forceinline__ float4 ld_shared_v4(uint32_t addr) {
     float4 v;
     asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(addr) : "memory");
+    return v;
+}
+__device__ __forceinline__ uint32_t ld_shared_u32(uint32_t addr) {
+    uint32_t v;
+    asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr) : "memory");
     return v;
 }
 

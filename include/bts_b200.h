@@ -134,16 +134,15 @@ int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int
                     int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                     const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
                     int act, int precision, double *stat_sum, double *stat_sumsq, int flags, void *stream);
-/* Staging of the activation tiles of bts_conv_fwd*: 0 = the producer warps load them (LDG + hi/lo split in registers),
+/* Staging of the activation tiles of bts_conv_fwd*: 0 = the producer warps load them (LDG + pre-op in registers),
  * 1 = TMA im2col loads (cp.async.bulk.tensor im2col; zero padding by out-of-bounds fill) land the raw tile in
- * shared memory as the A_hi operand and the producers only derive A_lo in place -- used for stride-1, non-up-sampled layers
+ * shared memory as the A operand and the producers only apply the pre-op in place -- used for stride-1, non-up-sampled layers
  * whose K channels are a multiple of 32 and whose rows are 16-byte aligned, every other layer keeps mode 0 automatically.
  * (2, 3: bring-up variants.)  Process-wide setting. */
 int bts_conv_set_tma(int mode);
 int bts_conv_get_tma(void);
-/* activation-producer groups of the conv engine (4 warps each): 0 / 4 = four groups without register prefetch on narrow
- * tiles (<= 48 output channels) whose operand ring has >= 4 stages (default), 2 = always two groups with one k-block of
- * register prefetch. */
+/* activation-producer groups of the conv engine (4 warps each): the engine runs two groups; 0 (default) and 2 are
+ * accepted, any other value returns BTS_EINVAL. */
 int bts_conv_set_producer_groups(int groups);
 /* Tuning / bring-up switches of the narrow-output wgrad (csrc/wgrad2_tc.cu).  set_tma(0): the producers load the operands
  * from global memory (round-1 path) instead of the TMA landing ring; set_min_pixels(n): smallest map (input pixels) routed to
