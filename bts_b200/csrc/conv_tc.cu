@@ -570,9 +570,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
 #pragma unroll
                         for (int j = 0; j < 4; ++j) {                      // j: row + 8 (j & 1), column + 4 (j >> 1)
                             const uint32_t x = ld_shared_u32((aF ^ (uint32_t)(32 * k + 16 * (j >> 1))) + 1024u * (j & 1));
-                            const uint32_t h = (x + 0x1000u) & 0xffffe000u;
-                            hi[k][j] = h;
-                            lo[k][j] = __float_as_uint(__uint_as_float(x) - __uint_as_float(h));
+                            float h, l;
+                            split_tf32(__uint_as_float(x), h, l);
+                            hi[k][j] = __float_as_uint(h);
+                            lo[k][j] = __float_as_uint(l);
                         }
                     }
                     wgmma_fence();

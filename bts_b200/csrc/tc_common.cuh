@@ -96,6 +96,14 @@ __device__ __forceinline__ float rna_tf32(float x) {
     return __uint_as_float(r);
 }
 
+// 3xTF32 operand split x = hi + lo: hi = x rounded to tf32 (round-half-away on the 13 dropped mantissa bits, two integer
+// ops), lo = x - hi, exact in fp32.  The tensor cores read the top 19 bits of each word, so hi*hi + hi*lo + lo*hi leaves
+// about 2^-21 relative per product.
+__device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
+    hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+    lo = x - hi;
+}
+
 struct __align__(16) F4 { float v[4]; };
 
 // Division of n < 2^31 by a runtime constant d >= 1 as multiply-high + shift (the divisor's magic numbers are computed

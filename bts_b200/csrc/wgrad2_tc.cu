@@ -388,12 +388,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
         auto split_store = [&](uint32_t hi_addr, uint32_t lo_addr, const F4 &v) {
             float hi[4], lo[4];
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                const float a = v.v[e];
-                const float hh = __uint_as_float((__float_as_uint(a) + 0x1000u) & 0xffffe000u);
-                hi[e] = hh;
-                lo[e] = a - hh;
-            }
+            for (int e = 0; e < 4; ++e) split_tf32(v.v[e], hi[e], lo[e]);
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 st_shared_f32(hi_addr + 16u * e, hi[e]);

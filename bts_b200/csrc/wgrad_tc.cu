@@ -3,12 +3,15 @@
 //   dW[co, ci, tap] = sum_p  dY[p, co] * pre(x[p (+) tap, ci])            (same pre / (+) as conv_tc.cu)
 //
 // GEMM view per (tap, split):  M = 128 input channels (two consumer warpgroups of 64), N = n_tile <= 64 output channels,
-// K = output pixels.  Both operands live in memory as [pixel][channel] (NHWC), i.e. the reduction index is the slow one,
-// while tf32 wgmma reads only K-major operands: the producers transpose on their way into shared memory, writing
-// [channel][pixel] tiles of 8 x 16-byte core matrices (no swizzle).
+// K = output pixels.  Both operands live in memory as [pixel][channel] (NHWC), i.e. the reduction index is the slow one.
+//   A = x: staged once per k-block as fp32 in its NHWC order ([pixel][channel], pre-op and zero padding applied); every
+//       consumer thread loads its tf32 fragments from it, splits them into hi/lo in registers and issues register-A wgmma.
+//   B = dY: tf32 wgmma reads shared-memory operands K-major only, so the producers transpose dY on its way into shared
+//       memory, split into hi/lo tiles of 8 x 16-byte core matrices (no swizzle).
 // grid = (ceil(Cin/128), n_tiles(Cout), taps * splitK); each CTA reduces its pixel range into fp32 register accumulators
 // and writes a partial; a second, deterministic kernel sums the splitK partials into the (Cout,Cin,KH,KW)-strided gradient.
-// 768 threads: 2 consumer warpgroups + 2 producer groups of 8 warps (x tile / dY tile), 2-4 operand stages.
+// 512 threads (16 warps, 128 registers per thread): 2 consumer warpgroups + 2 producer warpgroups (x tile / dY tile),
+// 2-6 operand stages.
 #include <cstdlib>
 #include <type_traits>
 
@@ -21,12 +24,13 @@ namespace {
 constexpr int BLOCK_CI = 128;
 constexpr int BLOCK_KP = 32;                 // pixels per k-block
 constexpr int MAX_N = 64;                    // output channels per CTA tile (register accumulator of the consumers)
-constexpr int MAX_STAGES = 4;
+constexpr int MAX_STAGES = 6;
 constexpr int SMEM_LIMIT = 232448;
 constexpr uint32_t CORE_SBO = 8 * 128 + 16;  // one 8-channel group of a k-block: 8 core matrices along K + a bank pad
-constexpr int A_BYTES = 16 * CORE_SBO;       // 128 channels (hi or lo)
+constexpr int X_ROW_BYTES = BLOCK_CI * 4;    // one pixel of the x tile: 128 fp32 channels
+constexpr int X_BYTES = BLOCK_KP * X_ROW_BYTES;
 constexpr int CONSUMER_THREADS = 256;
-constexpr int GROUP_THREADS = 256;
+constexpr int GROUP_THREADS = 128;
 constexpr int NUM_THREADS = CONSUMER_THREADS + 2 * GROUP_THREADS;
 
 struct WgradParams {
@@ -42,8 +46,9 @@ struct WgradParams {
     int splitK, kb_per_split, KBp;
     int M;
     int x_vec, dy_vec, precision;
-    int stages, stage_bytes;     // operand ring: [A hi | A lo | dY hi b_bytes | dY lo b_bytes] per stage
+    int stages, stage_bytes;     // operand ring: [x X_BYTES | dY hi b_bytes | dY lo b_bytes] per stage
     int b_bytes;
+    FastDiv fd_wout, fd_hout;
 };
 
 
@@ -86,18 +91,26 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             s_shift[c] = ch < p.Cin ? p.pre_shift[ch] : 0.f;
         }
     }
-    // channel chunks beyond the last live input / output channel are never produced: zero every stage once
-    for (int i = threadIdx.x; i < S * stage_bytes / 16; i += NUM_THREADS) st_shared_v4(base + i * 16, 0.f, 0.f, 0.f, 0.f);
-    fence_proxy_async();
+    // (no zero fill of the stages: the producers write every byte of a stage that is read, dead channels as zeros)
     __syncthreads();
 
     if (warp < CONSUMER_THREADS / 32) {
-        // ---- consumers: two warpgroups, input channels [64 wg, 64 wg + 64) of the tile; 3xTF32 per k8 step, small
-        //      cross terms first; a stage is released as soon as its wgmma group has completed (the other warpgroup keeps
-        //      the tensor cores busy meanwhile)
+        // ---- consumers: two warpgroups, input channels [64 wg, 64 wg + 64) of the tile.  Per k-block every thread loads
+        //      its A fragments from the fp32 x tile, splits them into hi/lo in registers (split_tf32) and issues per k8 step
+        //      A_lo*B_hi, A_hi*B_lo, A_hi*B_hi (small cross terms first), B hi/lo from shared memory; a stage is released as
+        //      soon as its wgmma group has completed (the other warpgroup keeps the tensor cores busy meanwhile)
         const int wg = warp >> 2;
-        const uint32_t b_off = 2 * A_BYTES;
+        const uint32_t b_off = X_BYTES;
         const uint32_t bl_off = b_off + (uint32_t)p.b_bytes;
+        // A fragment of k8 step k (wgmma_tf32.cuh): rows = channels c, c + 8 with c = 64 wg + 16 (warp % 4) + lane / 4,
+        // columns = pixels 8k + q, 8k + q + 4 with q = lane % 4.  Pixel r of the x tile is the 512-byte row r, its 16-byte
+        // chunk u (channels 4u..4u+3) stored at chunk u ^ 2 (r % 4): the 8 channels x 4 pixels of one fragment load hit 32
+        // distinct banks.  r % 4 == q for every fragment of the thread, and chunk(c + 8) = chunk(c) ^ 2 (c % 16 < 8), so
+        // channel c + 8 sits at byte offset aF ^ 32.
+        const int q = lane & 3;
+        const int c = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const uint32_t aF = (uint32_t)q * X_ROW_BYTES + ((uint32_t)((c >> 2) ^ (2 * q)) << 4) + (uint32_t)(c & 3) * 4u;
+        const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             float acc[N / 2];
@@ -107,30 +120,44 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             uint32_t ph = 0;
             for (int it = 0; it < nkb; ++it) {
                 mbar_wait(full(s), ph);
-                wgmma_fence();
                 const uint32_t st = base + (uint32_t)s * stage_bytes;
-                const uint32_t a_hi = st + (uint32_t)wg * 8u * CORE_SBO;
+                uint32_t hi[BLOCK_KP / 8][4], lo[BLOCK_KP / 8][4];
 #pragma unroll
-                for (int kg = 0; kg < BLOCK_KP / 8; ++kg) {
-                    const uint32_t ko = (uint32_t)kg * 256u;
-                    const uint64_t dah = make_desc_core(a_hi + ko, 128, CORE_SBO), dal = make_desc_core(a_hi + A_BYTES + ko, 128, CORE_SBO);
+                for (int k = 0; k < BLOCK_KP / 8; ++k) {
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {                      // j: row + 8 (j & 1), column + 4 (j >> 1)
+                        const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                        float h, l;
+                        split_tf32(__uint_as_float(x), h, l);
+                        hi[k][j] = __float_as_uint(h);
+                        lo[k][j] = __float_as_uint(l);
+                    }
+                }
+                wgmma_fence();
+#pragma unroll
+                for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                    const uint32_t ko = (uint32_t)k * 256u;
                     const uint64_t dbh = make_desc_core(st + b_off + ko, 128, CORE_SBO), dbl = make_desc_core(st + bl_off + ko, 128, CORE_SBO);
-                    const uint32_t accumulate = (it | kg) != 0;
-                    if (p.precision != 0) {
-                        Wgmma<N>::mma(acc, dah, dbh, accumulate);
+                    const uint32_t accumulate = (it | k) != 0;
+                    if (single) {
+                        Wgmma<N>::mma_rs(acc, hi[k], dbh, accumulate);
                     } else {
-                        Wgmma<N>::mma(acc, dal, dbh, accumulate);
-                        Wgmma<N>::mma(acc, dah, dbl, 1);
-                        Wgmma<N>::mma(acc, dah, dbh, 1);
+                        Wgmma<N>::mma_rs(acc, lo[k], dbh, accumulate);
+                        Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
+                        Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
                     }
                 }
                 wgmma_commit();
                 wgmma_wait<0>();
+                wgmma_fence_operands(acc);
+#pragma unroll
+                for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                    wgmma_fence_operands(hi[k]);
+                    wgmma_fence_operands(lo[k]);
+                }
                 mbar_arrive(empty(s));
                 if (++s == S) { s = 0; ph ^= 1; }
             }
-            wgmma_wait<0>();
-            wgmma_fence_operands(acc);
             // ---- epilogue: accumulator row = input channel, column = output channel; partial [split][tap][ci][co]
             const int taps = p.KH * p.KW;
             const bool ovec = (p.Cout & 1) == 0 && ((((uintptr_t)p.part) & 7) == 0) && (n_tile & 1) == 0;
@@ -161,105 +188,54 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             default: consume(std::integral_constant<int, 64>()); break;
         }
     } else {
-        // 8 warps per group (round 1 ran 4 with two pixel rows per thread: ~9 cycles between a warp's instructions at
-        // 2.5 warps per scheduler made the producers, not the tensor pipe, set the k-block time): one pixel row of the
-        // 32-pixel k-block per thread, 4 sixteen-byte units (one per 32-channel chunk).
+        // ---- producers: group 0 (warps 8..11) stages the x tiles, group 1 (warps 12..15) the dY tiles; each keeps the
+        //      global loads of its next k-block in flight while it stores the current one (register ping-pong)
         const int pt = threadIdx.x - CONSUMER_THREADS;
-        const int grp = pt >> 8;                   // group 0 produces the x (A) tiles, group 1 the dY (B) tiles
-        const int t = pt & 255;
-        const int unit = t & 7;                    // 16-byte unit of the 128-byte row
-        const int r0 = t >> 3;                     // pixel row r0 of the 32-pixel k-block
+        const int grp = pt / GROUP_THREADS;
+        const int t = pt % GROUP_THREADS;
         constexpr bool AFF = PRE >= 2;
         constexpr bool RELU = (PRE & 1) != 0;
-        constexpr int NU = 4;                      // units per thread per k-block
-        // K-major core-matrix tiles: element (row = channel, k = pixel) at (row / 8) * CORE_SBO + (k / 4) * 128 +
-        // (row % 8) * 16 + (k % 4) * 4.  A thread holds 4 consecutive channels of one pixel: 4 scalar stores, which the
-        // 16-byte pad of CORE_SBO spreads over all 32 banks across the warp.
-        uint32_t roff[NU];
-#pragma unroll
-        for (int i = 0; i < NU; ++i)
-            roff[i] = (uint32_t)(i * 4 + (unit >> 1)) * CORE_SBO + (uint32_t)(r0 >> 2) * 128u + (uint32_t)(unit & 1) * 64u +
-                      (uint32_t)(r0 & 3) * 4u;
-
-        // hi/lo split + swizzled stores of up to 8 units (4 chunks x 2 rows); only `nlive` chunks are written
-        // (the A regions were zeroed once, so dead channel chunks stay zero)
-        auto split_store = [&](uint32_t t_hi, uint32_t t_lo, F4(&v)[NU], int nlive) {
-#pragma unroll
-            for (int i = 0; i < NU; ++i) {
-                if (i < nlive) {
-                    float hi[4], lo[4];
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        const float a = v[i].v[e];
-                        const float hh = __uint_as_float((__float_as_uint(a) + 0x1000u) & 0xffffe000u);
-                        hi[e] = hh;
-                        lo[e] = a - hh;
-                    }
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        st_shared_f32(t_hi + roff[i] + 16u * e, hi[e]);
-                        st_shared_f32(t_lo + roff[i] + 16u * e, lo[e]);
-                    }
-                }
-            }
-        };
 
         if (grp == 0) {
-            // ------------------------------ x tiles (A operand): 4 chunks of 32 input channels ------------------
+            // ------------------------------ x tiles (A operand), fp32 [pixel][channel] --------------------------------
+            // Thread t owns the 4-channel unit u = t % 32 of pixel rows r0 + 4 i (i = 0..7, r0 = t / 32): a warp reads one
+            // pixel's 512 contiguous bytes per row and writes them with one 128-bit shared store per lane (the chunk
+            // swizzle u ^ 2 r0 permutes chunks within aligned groups of 8: conflict-free).
+            constexpr int NR = BLOCK_KP / 4;           // rows per thread per k-block
+            const int u = t & 31, r0 = t >> 5;
+            const uint32_t xoff = (uint32_t)r0 * X_ROW_BYTES + ((uint32_t)(u ^ (2 * r0)) << 4);   // + 4 i rows
             const int Hin = UP ? 2 * p.Hs : p.Hs, Win = UP ? 2 * p.Ws : p.Ws;
             const int dyo = (tap / p.KW) * p.dil - p.pad, dxo = (tap % p.KW) * p.dil - p.pad;
             const int xs = (int)p.xs;
-            const int cb = ci_tile * BLOCK_CI + unit * 4;
-            int nlive = (p.Cin - ci_tile * BLOCK_CI + 31) >> 5;      // chunks that hold real channels
-            if (nlive > 4) nlive = 4;
-            float sc[4][4], sh[4][4];
+            const int c = ci_tile * BLOCK_CI + u * 4;  // first input channel of the unit
+            float sc[4], sh[4];
             if (AFF) {
 #pragma unroll
-                for (int ch = 0; ch < 4; ++ch)
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        sc[ch][e] = s_scale[ch * 32 + unit * 4 + e];
-                        sh[ch][e] = s_shift[ch * 32 + unit * 4 + e];
-                    }
+                for (int e = 0; e < 4; ++e) {
+                    sc[e] = s_scale[u * 4 + e];        // 0 beyond Cin
+                    sh[e] = s_shift[u * 4 + e];
+                }
             }
             const float *__restrict__ xg = p.x;
-            // output-pixel coordinates of this thread's two rows, advanced by 32 pixels per k-block (no divisions)
-            int px[1], py[1], pb[1];
+            auto load_x = [&](int it, F4(&v)[NR], uint32_t &mask) {
+                const int m0 = (kb0 + it) * BLOCK_KP + r0;
+                uint32_t mk = 0;
 #pragma unroll
-            for (int h = 0; h < 1; ++h) {
-                const int m = kb0 * BLOCK_KP + r0;
-                px[h] = m % p.Wout;
-                const int q = m / p.Wout;
-                py[h] = q % p.Hout;
-                pb[h] = q / p.Hout;
-            }
-            auto load_x = [&](int it, F4(&v)[NU], uint32_t &mask) {
-                const int kb = kb0 + it;
-                int off[1];
-                bool ok[1];
-#pragma unroll
-                for (int h = 0; h < 1; ++h) {
-                    const int m = kb * BLOCK_KP + r0;
-                    const int yy = py[h] * p.stride + dyo, xx = px[h] * p.stride + dxo;
-                    ok[h] = m < p.M && (unsigned)yy < (unsigned)Hin && (unsigned)xx < (unsigned)Win;
+                for (int i = 0; i < NR; ++i) {
+                    const int m = m0 + 4 * i;
+                    const uint32_t qo = fdiv((uint32_t)m, p.fd_wout);
+                    const uint32_t b = fdiv(qo, p.fd_hout);
+                    const int ox = m - (int)qo * p.Wout, oy = (int)qo - (int)b * p.Hout;
+                    const int yy = oy * p.stride + dyo, xx = ox * p.stride + dxo;
+                    const bool ok = m < p.M && (unsigned)yy < (unsigned)Hin && (unsigned)xx < (unsigned)Win;
+                    mk |= (ok ? 1u : 0u) << i;
                     const int sy = UP ? (yy >> 1) : yy, sx = UP ? (xx >> 1) : xx;
-                    off[h] = ((pb[h] * p.Hs + sy) * p.Ws + sx) * xs + cb;
-                    px[h] += BLOCK_KP;
-                    while (px[h] >= p.Wout) {
-                        px[h] -= p.Wout;
-                        if (++py[h] == p.Hout) { py[h] = 0; ++pb[h]; }
-                    }
-                }
-                mask = ok[0] ? 1u : 0u;
-#pragma unroll
-                for (int i = 0; i < NU; ++i) {
-                    const int h = 0, chunk = i;
-                    const int c = cb + chunk * 32;
-                    const bool live = chunk < nlive && ok[h] && c < p.Cin;
+                    const int off = (((int)b * p.Hs + sy) * p.Ws + sx) * xs + c;
+                    const bool live = ok && c < p.Cin;
                     if (VEC) {
                         float4 q4 = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (live) q4 = __ldg(reinterpret_cast<const float4 *>(xg + off[h] + chunk * 32));
-                        if (c + 3 >= p.Cin) {        // channel tail of a 16-byte-padded row
+                        if (live) q4 = __ldg(reinterpret_cast<const float4 *>(xg + off));
+                        if (c + 3 >= p.Cin) {          // channel tail of a 16-byte-padded row
                             if (c + 1 >= p.Cin) q4.y = 0.f;
                             if (c + 2 >= p.Cin) q4.z = 0.f;
                             q4.w = 0.f;
@@ -269,65 +245,73 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
 #pragma unroll
                         for (int e = 0; e < 4; ++e) {
                             float q1 = 0.f;
-                            if (live && c + e < p.Cin) q1 = __ldg(xg + off[h] + chunk * 32 + e);
+                            if (live && c + e < p.Cin) q1 = __ldg(xg + off + e);
                             v[i].v[e] = q1;
                         }
                     }
                 }
+                mask = mk;
             };
             int xs_s = 0;
             uint32_t xs_ph = 0;
-            auto store_x = [&](int it, F4(&v)[NU], uint32_t mask) {
-                const int s = xs_s;
-                const uint32_t ph = xs_ph;
-                if (++xs_s == S) { xs_s = 0; xs_ph ^= 1; }
+            auto store_x = [&](F4(&v)[NR], uint32_t mask) {
                 if (PRE != 0) {
 #pragma unroll
-                    for (int i = 0; i < NU; ++i)
+                    for (int i = 0; i < NR; ++i)
 #pragma unroll
                         for (int e = 0; e < 4; ++e) {
                             float a = v[i].v[e];
                             if (AFF) {
-                                a = fmaf(a, sc[i][e], sh[i][e]);
+                                a = fmaf(a, sc[e], sh[e]);
                                 if (RELU) a = fmaxf(a, 0.f);
-                                a = (mask & 1u) ? a : 0.f;
+                                a = ((mask >> i) & 1u) ? a : 0.f;     // zero padding is applied after the pre-op
                             } else {
                                 a = fmaxf(a, 0.f);
                             }
                             v[i].v[e] = a;
                         }
                 }
-                mbar_wait(empty(s), ph ^ 1);
-                const uint32_t t_hi = base + (uint32_t)s * stage_bytes;
-                split_store(t_hi, t_hi + A_BYTES, v, nlive);
-                fence_proxy_async();
-                mbar_arrive(full(s));
+                mbar_wait(empty(xs_s), xs_ph ^ 1);
+                const uint32_t dst = base + (uint32_t)xs_s * stage_bytes + xoff;
+#pragma unroll
+                for (int i = 0; i < NR; ++i)
+                    st_shared_v4(dst + (uint32_t)(4 * i) * X_ROW_BYTES, v[i].v[0], v[i].v[1], v[i].v[2], v[i].v[3]);
+                mbar_arrive(full(xs_s));               // the consumers read x with generic loads: no proxy fence
+                if (++xs_s == S) { xs_s = 0; xs_ph ^= 1; }
             };
-            F4 va[NU], vb[NU];
+            F4 va[NR], vb[NR];
             uint32_t ma = 0, mb = 0;
             int it = 0;
             if (it < nkb) load_x(it, va, ma);
             for (; it < nkb; it += 2) {
                 const bool more = it + 1 < nkb;
                 if (more) load_x(it + 1, vb, mb);
-                store_x(it, va, ma);
+                store_x(va, ma);
                 if (more) {
                     if (it + 2 < nkb) load_x(it + 2, va, ma);
-                    store_x(it + 1, vb, mb);
+                    store_x(vb, mb);
                 }
             }
         } else {
             // ------------------------------ dY tiles (B operand): ceil(n_tile/32) <= 2 chunks of output channels ---
+            // Thread t owns the 4-channel unit `unit` = t % 8 of each chunk in pixel rows r0 and r0 + 16 (r0 = t / 8).
+            // K-major core-matrix tiles: element (row = channel, k = pixel) at (row / 8) * CORE_SBO + (k / 4) * 128 +
+            // (row % 8) * 16 + (k % 4) * 4.  A unit is 4 scalar stores, which the 16-byte pad of CORE_SBO spreads over all
+            // 32 banks across the warp.
+            const int unit = t & 7, r0 = t >> 3;
+            const uint32_t roff = (uint32_t)(unit >> 1) * CORE_SBO + (uint32_t)(r0 >> 2) * 128u + (uint32_t)(unit & 1) * 64u +
+                                  (uint32_t)(r0 & 3) * 4u;   // + chunk * 4 CORE_SBO + h * 512 for row r0 + 16 h
             const int dys = (int)p.dys;
             const int nchunk = (n_tile + 31) >> 5;
             const int cb = nt * n_tile + unit * 4;
             const float *__restrict__ dg = p.dy;
+            constexpr int NU = 4;                      // v[2 h + chunk]
             auto load_d = [&](int it, F4(&v)[NU]) {
                 const int kb = kb0 + it;
 #pragma unroll
                 for (int i = 0; i < NU; ++i) {
-                    const int chunk = i;
-                    const int m = kb * BLOCK_KP + r0;
+                    const int h = i >> 1, chunk = i & 1;
+                    const int m = kb * BLOCK_KP + r0 + 16 * h;
                     const int c = cb + chunk * 32;
                     const bool live = chunk < nchunk && m < p.M && c < p.Cout;
                     if (VEC) {
@@ -352,29 +336,41 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             int ds_s = 0;
             uint32_t ds_ph = 0;
             auto store_d = [&](F4(&v)[NU]) {
-                const int s = ds_s;
-                mbar_wait(empty(s), ds_ph ^ 1);
-                const uint32_t t_hi = base + (uint32_t)s * stage_bytes + 2 * A_BYTES;
-                split_store(t_hi, t_hi + (uint32_t)p.b_bytes, v, nchunk);
-                fence_proxy_async();
-                mbar_arrive(full(s));
+                mbar_wait(empty(ds_s), ds_ph ^ 1);
+                const uint32_t t_hi = base + (uint32_t)ds_s * stage_bytes + X_BYTES + roff;
+                const uint32_t t_lo = t_hi + (uint32_t)p.b_bytes;
+#pragma unroll
+                for (int i = 0; i < NU; ++i) {
+                    const int h = i >> 1, chunk = i & 1;
+                    if (chunk < nchunk) {
+                        const uint32_t o = (uint32_t)chunk * 4u * CORE_SBO + (uint32_t)h * 512u;
+                        float hi[4], lo[4];
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) split_tf32(v[i].v[e], hi[e], lo[e]);
+#pragma unroll
+                        for (int e = 0; e < 4; ++e) {
+                            st_shared_f32(t_hi + o + 16u * e, hi[e]);
+                            st_shared_f32(t_lo + o + 16u * e, lo[e]);
+                        }
+                    }
+                }
+                fence_proxy_async();                   // generic-proxy writes -> visible to wgmma (async proxy)
+                mbar_arrive(full(ds_s));
                 if (++ds_s == S) { ds_s = 0; ds_ph ^= 1; }
             };
             F4 va[NU], vb[NU];
-            const int nj = nkb;
             int it = 0;
-            if (it < nj) load_d(it, va);
-            for (; it < nj; it += 2) {
-                const bool more = it + 1 < nj;
+            if (it < nkb) load_d(it, va);
+            for (; it < nkb; it += 2) {
+                const bool more = it + 1 < nkb;
                 if (more) load_d(it + 1, vb);
                 store_d(va);
                 if (more) {
-                    if (it + 2 < nj) load_d(it + 2, va);
+                    if (it + 2 < nkb) load_d(it + 2, va);
                     store_d(vb);
                 }
             }
         }
-
     }
 }
 
@@ -501,6 +497,8 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     p.x_vec = bts_aligned16(x) && (x_pixel_stride % 4 == 0);
     p.dy_vec = bts_aligned16(dy) && (dy_pixel_stride % 4 == 0);
     p.precision = precision;
+    p.fd_wout = make_fastdiv((uint32_t)p.Wout);
+    p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     const int taps = KH * KW;
     if (bts_wgrad2_eligible(Cout, KH, KW, stride, M)) {
         int rc2 = bts_wgrad2_launch(x, x_pixel_stride, B, Hs, Ws, p.up, Cin, KH, KW, pad, dil, pre_scale, pre_shift,
@@ -519,7 +517,7 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     {
         const int nchunk = (p.n_tile + 31) / 32;
         p.b_bytes = nchunk * 4 * (int)CORE_SBO;
-        p.stage_bytes = 2 * A_BYTES + 2 * p.b_bytes;
+        p.stage_bytes = X_BYTES + 2 * p.b_bytes;
         p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
         if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
         if (p.stages < 2) return BTS_EINVAL;
@@ -626,9 +624,11 @@ extern "C" int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, 
     p.x_vec = bts_aligned16(x) && (x_pixel_stride % 4 == 0);
     p.dy_vec = bts_aligned16(dy) && (dy_pixel_stride % 4 == 0);
     p.precision = precision;
+    p.fd_wout = make_fastdiv((uint32_t)p.Wout);
+    p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     const int taps = KH * KW;
     p.b_bytes = 2 * 4 * (int)CORE_SBO;
-    p.stage_bytes = 2 * A_BYTES + 2 * p.b_bytes;
+    p.stage_bytes = X_BYTES + 2 * p.b_bytes;
     p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     const int smem = p.stages * p.stage_bytes + 2 * BLOCK_CI * 4 + 256 + 1024;
