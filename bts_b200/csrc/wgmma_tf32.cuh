@@ -1,6 +1,6 @@
-// wgmma wrappers (sm_90a): D[64 x N] (+)= A[64 x 8] * B[8 x N]^T, fp32 accumulators in registers, tf32 operands read
-// from shared memory through matrix descriptors (K-major: the only layout wgmma accepts for tf32).  mma: A and B from
-// shared memory (SS); mma_rs: A from registers, B from shared memory (RS).
+// wgmma wrappers (sm_90a): D[64 x N] (+)= A[64 x 8] * B[8 x N]^T, fp32 accumulators in registers, tf32 operands.
+// mma_rs: A from registers, B from shared memory through a matrix descriptor (K-major: the only layout wgmma accepts for
+// tf32).
 //
 // A fragment of mma_rs, thread t (warp w = t / 32, lane l, g = l / 4, q = l % 4): a[0] = (row 16 w + g, column q),
 // a[1] = (row + 8, q), a[2] = (row, q + 4), a[3] = (row + 8, q + 4) of the k8 step; the tensor core reads the top 19 bits
@@ -16,13 +16,6 @@ namespace tc {
 template <int N> struct Wgmma;
 
 template <> struct Wgmma<16> {
-    static __device__ __forceinline__ void mma(float (&d)[8], uint64_t a, uint64_t b, uint32_t scale_d) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, p, 1, 1;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
-            : "l"(a), "l"(b), "r"(scale_d));
-    }
     static __device__ __forceinline__ void mma_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
@@ -33,13 +26,6 @@ template <> struct Wgmma<16> {
 };
 
 template <> struct Wgmma<32> {
-    static __device__ __forceinline__ void mma(float (&d)[16], uint64_t a, uint64_t b, uint32_t scale_d) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, p, 1, 1;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
-            : "l"(a), "l"(b), "r"(scale_d));
-    }
     static __device__ __forceinline__ void mma_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
@@ -50,13 +36,6 @@ template <> struct Wgmma<32> {
 };
 
 template <> struct Wgmma<48> {
-    static __device__ __forceinline__ void mma(float (&d)[24], uint64_t a, uint64_t b, uint32_t scale_d) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %26, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23}, %24, %25, p, 1, 1;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
-            : "l"(a), "l"(b), "r"(scale_d));
-    }
     static __device__ __forceinline__ void mma_rs(float (&d)[24], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %29, 0;\n\t"
@@ -67,13 +46,6 @@ template <> struct Wgmma<48> {
 };
 
 template <> struct Wgmma<64> {
-    static __device__ __forceinline__ void mma(float (&d)[32], uint64_t a, uint64_t b, uint32_t scale_d) {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1;\n\t}"
-            : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
-            : "l"(a), "l"(b), "r"(scale_d));
-    }
     static __device__ __forceinline__ void mma_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
         asm volatile(
             "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
@@ -84,12 +56,12 @@ template <> struct Wgmma<64> {
 };
 
 template <> struct Wgmma<80> {
-    static __device__ __forceinline__ void mma(float (&d)[40], uint64_t a, uint64_t b, uint32_t scale_d) {
+    static __device__ __forceinline__ void mma_rs(float (&d)[40], const uint32_t (&a)[4], uint64_t b, uint32_t scale_d) {
         asm volatile(
-            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %42, 0;\n\t"
-            "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, %40, %41, p, 1, 1;\n\t}"
+            "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %45, 0;\n\t"
+            "wgmma.mma_async.sync.aligned.m64n80k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39}, {%40, %41, %42, %43}, %44, p, 1, 1;\n\t}"
             : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39])
-            : "l"(a), "l"(b), "r"(scale_d));
+            : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b), "r"(scale_d));
     }
 };
 

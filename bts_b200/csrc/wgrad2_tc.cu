@@ -6,17 +6,21 @@
 //
 // wgrad_tc.cu puts the tap in the grid, so the activation tile -- the expensive operand: loads, BN/ReLU pre-op, hi/lo
 // split, shared-memory writes per k-block -- is produced once per tap.  Here ONE CTA owns all taps of a (64 ci, cg co)
-// block: per k-block of 16 input pixels the activation tile is produced once and multiplied against the shifted dY tiles
+// block: per k-block of 32 input pixels the activation tile is produced once and multiplied against the shifted dY tiles
 // of every tap, packed densely along N (tap t owns the N slots [t*ncol, (t+1)*ncol)), so that wgmma of width
 // taps*ncol <= 144 covers them all; two consumer warpgroups split those columns (<= 40 accumulator registers per thread).
-// Operand tiles are K-major (pixels contiguous per channel row) in 8 x 16-byte core matrices, written by the producers;
-// deterministic split-K partial layout as wgrad_tc.cu.
+//   A = x: staged once per k-block as fp32 in its NHWC order ([pixel][64 channels], pre-op and zero padding applied);
+//       every consumer thread loads its tf32 fragments from it, splits them into hi/lo in registers and issues
+//       register-A wgmma.
+//   B = dY: K-major (pixels contiguous per column) hi/lo tiles of 8 x 16-byte core matrices, transposed by the producers.
+// Deterministic split-K partial layout as wgrad_tc.cu; split-K ranges are whole multiples of 16 pixels.
+// 512 threads (16 warps, 128 registers per thread): 2 consumer warpgroups + 2 producer warpgroups.
 //
-// Operand staging: the shifted dY windows of a k-block overlap -- they are KH row segments of 16 + (KW-1)*dil consecutive
-// output pixels.  With TMA = true a loader lane copies the raw fp32 segments (and the raw x tile unless it is read through
-// the nearest-neighbour up-sample) into a small landing ring, several k-blocks ahead (cp.async.bulk.tensor.2d, no swizzle,
-// zero fill past the tensor ends); the producers then read shared memory, apply the border masks / pre-op, split hi/lo
-// and write the operand tiles.
+// Operand staging: the shifted dY windows of a k-block overlap -- they are KH row segments of 32 + (KW-1)*dil consecutive
+// output pixels.  With TMA = true one producer lane copies the raw fp32 segments (and the raw x tile unless it is read
+// through the nearest-neighbour up-sample) into a small landing ring, `ring` k-blocks ahead (cp.async.bulk.tensor.2d, no
+// swizzle, zero fill past the tensor ends); the producers then read shared memory, apply the border masks / pre-op and
+// write the operand tiles.
 #include <cuda.h>
 
 #include <cstring>
@@ -29,21 +33,20 @@ using namespace tc;
 namespace {
 
 constexpr int BLOCK_CI = 64;                 // input channels per CTA = the M of one consumer warpgroup
-constexpr int X_CHUNKS = BLOCK_CI / 32;      // 32-channel chunks of the activation tile
-constexpr int KP = 16;                       // input pixels per k-block (2 k-groups of 8)
-constexpr uint32_t CORE_SBO = 4 * 128 + 16;  // one 8-row group of a k-block: 4 core matrices along K + a bank pad
-constexpr int A_BYTES = BLOCK_CI / 8 * CORE_SBO;   // hi or lo
+constexpr int KP = 32;                       // input pixels per k-block (4 k8 steps)
+constexpr int SPLIT_PX = 16;                 // split-K ranges are whole multiples of this many pixels (bts_wgrad2_plan)
+constexpr uint32_t CORE_SBO = KP / 4 * 128 + 16;   // one 8-column group of a k-block: 8 core matrices along K + a bank pad
+constexpr int X_ROW_BYTES = BLOCK_CI * 4;    // one pixel of the x tile: 64 fp32 channels
+constexpr int X_BYTES = KP * X_ROW_BYTES;    // x tile of a k-block (stage and landing ring): 8 KB
 constexpr int MAX_TAPS = 9;
 constexpr int MAX_NT = 144;                  // widest packed N (taps * ncol), split between the two consumer warpgroups
+constexpr int MAX_CHUNKS = (MAX_NT + 31) / 32;   // 32-column chunks of the packed dY tile
 constexpr int MAX_STAGES = 4;
 constexpr int CONSUMER_THREADS = 256;       // two warpgroups, each owns about half of the packed N columns
-constexpr int LOADER_WARP = CONSUMER_THREADS / 32;
-constexpr int GROUPS = 3;                    // producer groups of 128 threads: group g owns the dY taps t == g (mod 3)
-constexpr int PRODUCERS = 128 * GROUPS;
-constexpr int NUM_THREADS = CONSUMER_THREADS + 32 + PRODUCERS;
+constexpr int PRODUCERS = 256;
+constexpr int NUM_THREADS = CONSUMER_THREADS + PRODUCERS;
 constexpr int SMEM_BUDGET = 224 * 1024;
 constexpr int MAX_RING = 4;                  // landing-ring slots (TMA staging)
-constexpr int X_RAW_BYTES = KP * BLOCK_CI * 4;   // raw x tile of a k-block: 4 KB
 
 struct W2Params {
     const float *x; long long xs;
@@ -52,12 +55,11 @@ struct W2Params {
     const float *pre_scale, *pre_shift;
     const float *dy; long long dys;
     int Cout, Hout, Wout, Hin, Win;
-    int cg, nb;              // output channels per CTA (multiple of 16) and their 32-channel chunks
-    int nchunks;             // 32-row chunks of the tap-packed dY tile: ceil(taps*cg/32)
+    int cg;                  // output channels per CTA (multiple of 16)
     float *part;             // [splitK][taps][Cin][Cout]
-    int splitK, kb_per_split, KBq;
+    int splitK, px_per_split;
     int Mq;                  // B*Hin*Win input pixels
-    int stages, stage_bytes, precision;
+    int stages, stage_bytes, b_half, precision;   // stage = [x X_BYTES | dY hi b_half | dY lo b_half]
     // TMA landing ring (TMA = true): slot = [raw x tile (unless up) | KH segments of segw pixels x cg channels]
     int ring, slot_bytes, seg_bytes, segw, tox_max, slot_tx;
 };
@@ -70,7 +72,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
     uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
     const int taps = p.KH * p.KW;
     const int S = p.stages;
-    const uint32_t ring_off = (uint32_t)S * (uint32_t)p.stage_bytes;
+    const uint32_t stage_bytes = (uint32_t)p.stage_bytes;
+    const uint32_t ring_off = (uint32_t)S * stage_bytes;
     const uint32_t pre_off = ring_off + (TMA ? (uint32_t)p.ring * (uint32_t)p.slot_bytes : 0u);
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + BLOCK_CI;
@@ -83,16 +86,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
     const int ci_tile = blockIdx.x, cgi = blockIdx.y, split = blockIdx.z;
     const int co0 = cgi * p.cg;
     const int ncol = min(p.cg, ((p.Cout - co0 + 15) >> 4) << 4);     // live columns of this CTA (multiple of 16)
-    const int nb = p.nb;
-    // dY operand: the taps are packed DENSELY along N -- tap t owns the N rows [t*ncol, (t+1)*ncol) of one tile of
-    // ceil(taps*ncol/32) 32-row chunks -- so that a single wgmma multiplies the activation tile against all taps at once.
-    // hi and lo tiles follow each other.
+    // dY operand: the taps are packed DENSELY along N -- tap t owns the N columns [t*ncol, (t+1)*ncol) -- so that a single
+    // wgmma multiplies the activation tile against all taps at once.  hi and lo tiles follow each other.
     const int n_total = taps * ncol;
-    const uint32_t b_half = (uint32_t)p.nchunks * 4u * CORE_SBO;
-    const int kb0 = split * p.kb_per_split;
-    int kb1 = kb0 + p.kb_per_split;
-    if (kb1 > p.KBq) kb1 = p.KBq;
-    const int nkb = kb1 > kb0 ? kb1 - kb0 : 0;
+    const int q_begin = split * p.px_per_split;                      // this CTA's input pixels [q_begin, q_end)
+    const int q_end = min(q_begin + p.px_per_split, p.Mq);
+    const int nkb = q_end > q_begin ? (q_end - q_begin + KP - 1) / KP : 0;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < MAX_STAGES; ++s) {
@@ -112,77 +111,77 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
             s_shift[c] = ch < p.Cin ? p.pre_shift[ch] : 0.f;
         }
     }
-    // zero every operand stage once: dead channel chunks / dead units are never written afterwards
-    for (int i = threadIdx.x; i < S * p.stage_bytes / 16; i += NUM_THREADS) st_shared_v4(base + i * 16, 0.f, 0.f, 0.f, 0.f);
-    fence_proxy_async();
+    // (no zero fill of the stages: the producers write every byte of a stage that is read, dead channels as zeros)
     __syncthreads();
 
-    if (warp == LOADER_WARP) {
-        // ---- loader: one lane keeps the landing ring `ring` k-blocks ahead of the producers
-        if (TMA && lane == 0) {
-            if (!UP) tma_prefetch_desc(&tmx);
-            tma_prefetch_desc(&tmd);
-            int j = 0;
-            uint32_t ph = 0;
-            for (int it = 0; it < nkb; ++it) {
-                mbar_wait(rempty(j), ph ^ 1);
-                const uint32_t dst = base + ring_off + (uint32_t)j * (uint32_t)p.slot_bytes;
-                const int q0 = (kb0 + it) * KP;
-                mbar_arrive_expect_tx(rfull(j), (uint32_t)p.slot_tx);
-                uint32_t seg = dst;
-                if (!UP) {
-                    tma_tile_2d(dst, &tmx, ci_tile * BLOCK_CI, q0, rfull(j));
-                    seg += X_RAW_BYTES;
-                }
-                for (int ky = 0; ky < p.KH; ++ky)     // output pixels q - (ky*dil - pad)*W - tox, tox <= tox_max
-                    tma_tile_2d(seg + (uint32_t)ky * (uint32_t)p.seg_bytes, &tmd, co0,
-                                q0 - (ky * p.dil - p.pad) * p.Wout - p.tox_max, rfull(j));
-                if (++j == p.ring) { j = 0; ph ^= 1; }
-            }
-        }
-    } else if (warp < LOADER_WARP) {
+    if (warp < CONSUMER_THREADS / 32) {
         // ---- consumer warpgroups: rows = the 64 input channels; warpgroup wg owns the packed columns [n0, n0 + N) of
-        //      all taps x ncol (n0 = 0 | the first half rounded up to 16); 3xTF32 per k8 step, small cross terms first;
-        //      a stage is released as soon as its wgmma group has completed
+        //      all taps x ncol (n0 = 0 | the first half rounded up to 16).  Per k-block every thread loads its A fragments
+        //      from the fp32 x tile, splits them into hi/lo in registers and issues per k8 step A_lo*B_hi, A_hi*B_lo,
+        //      A_hi*B_hi (small cross terms first); a stage is released as soon as its wgmma group has completed
         const int wg = warp >> 2;
         const int n_half = (n_total + 31) / 32 * 16;
         const int n0 = wg ? n_half : 0, n_mine = wg ? n_total - n_half : n_half;
+        // A fragment of k8 step k (wgmma_tf32.cuh): rows = channels c, c + 8 with c = 16 (warp % 4) + lane / 4, columns =
+        // pixels 8k + q, 8k + q + 4 with q = lane % 4.  Pixel r of the x tile is the 256-byte row r (64 banks: a multiple
+        // of 32), its 16-byte chunk u (channels 4u..4u+3) stored at chunk u ^ 2 (r % 4).  The 8 channels of one load span
+        // chunks u0, u0 + 1 (u0 = 4 (warp % 4), so u0 % 8 is 0 or 4); XOR-ing 2q into bits 1-2 sends the 4 pixels to the
+        // 4 distinct pairs of chunks mod 8, so the 8 channels x 4 pixels hit 32 distinct banks.  r % 4 == q for every
+        // fragment of the thread, and chunk(c + 8) = chunk(c) ^ 2 (c % 16 < 8), so channel c + 8 sits at byte offset aF ^ 32.
+        const int q = lane & 3;
+        const int c = (warp & 3) * 16 + (lane >> 2);
+        const uint32_t aF = (uint32_t)q * X_ROW_BYTES + ((uint32_t)((c >> 2) ^ (2 * q)) << 4) + (uint32_t)(c & 3) * 4u;
+        const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             float acc[N > 0 ? N / 2 : 1];
 #pragma unroll
             for (int i = 0; i < (N > 0 ? N / 2 : 1); ++i) acc[i] = 0.f;
-            const bool single = p.precision != 0;
             int s = 0;
             uint32_t ph = 0;
             for (int it = 0; it < nkb; ++it) {
                 mbar_wait(full(s), ph);
-                wgmma_fence();
-                const uint32_t a_hi = base + (uint32_t)s * (uint32_t)p.stage_bytes, a_lo = a_hi + A_BYTES;
-                const uint32_t b_hi = a_hi + 2 * A_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO, b_lo = b_hi + b_half;
                 if constexpr (N > 0) {
+                    const uint32_t st = base + (uint32_t)s * stage_bytes;
+                    uint32_t hi[KP / 8][4], lo[KP / 8][4];
 #pragma unroll
-                    for (int kg = 0; kg < KP / 8; ++kg) {
-                        const uint32_t ko = (uint32_t)kg * 256u;
-                        const uint64_t dah = make_desc_core(a_hi + ko, 128, CORE_SBO), dal = make_desc_core(a_lo + ko, 128, CORE_SBO);
-                        const uint64_t dbh = make_desc_core(b_hi + ko, 128, CORE_SBO), dbl = make_desc_core(b_lo + ko, 128, CORE_SBO);
-                        const uint32_t accumulate = (it | kg) != 0;
-                        if (single) {
-                            Wgmma<N>::mma(acc, dah, dbh, accumulate);
-                        } else {
-                            Wgmma<N>::mma(acc, dal, dbh, accumulate);
-                            Wgmma<N>::mma(acc, dah, dbl, 1);
-                            Wgmma<N>::mma(acc, dah, dbh, 1);
+                    for (int k = 0; k < KP / 8; ++k) {
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
+                            const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                            float h, l;
+                            split_tf32(__uint_as_float(x), h, l);
+                            hi[k][j] = __float_as_uint(h);
+                            lo[k][j] = __float_as_uint(l);
                         }
                     }
+                    const uint32_t b_hi = st + X_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO, b_lo = b_hi + (uint32_t)p.b_half;
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < KP / 8; ++k) {
+                        const uint32_t ko = (uint32_t)k * 256u;
+                        const uint64_t dbh = make_desc_core(b_hi + ko, 128, CORE_SBO), dbl = make_desc_core(b_lo + ko, 128, CORE_SBO);
+                        const uint32_t accumulate = (it | k) != 0;
+                        if (single) {
+                            Wgmma<N>::mma_rs(acc, hi[k], dbh, accumulate);
+                        } else {
+                            Wgmma<N>::mma_rs(acc, lo[k], dbh, accumulate);
+                            Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
+                            Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
+                        }
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_operands(acc);
+#pragma unroll
+                    for (int k = 0; k < KP / 8; ++k) {
+                        wgmma_fence_operands(hi[k]);
+                        wgmma_fence_operands(lo[k]);
+                    }
                 }
-                wgmma_commit();
-                wgmma_wait<0>();
                 mbar_arrive(empty(s));
                 if (++s == S) { s = 0; ph ^= 1; }
             }
-            wgmma_wait<0>();
-            wgmma_fence_operands(acc);
             if (N == 0) return;
             // ---- epilogue: accumulator row = input channel, column n = tap (n / ncol), output channel co0 + n % ncol
             const bool ovec = (p.Cout & 1) == 0 && ((((uintptr_t)p.part) & 7) == 0) && ((co0 & 1) == 0);
@@ -215,74 +214,67 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
             default: consume(std::integral_constant<int, 80>()); break;
         }
     } else {
-        // 12 producer warps in GROUPS = 3 groups of 128 threads.  Group q owns the x chunk q (if any) and the dY taps
-        // t == q (mod 3): at most 1 + 6 sixteen-byte units per thread.
-        const int pt = threadIdx.x - (CONSUMER_THREADS + 32);   // 0..PRODUCERS-1
-        const int unit = pt & 7;                   // 16-byte unit of the 128-byte row
-        const int row = (pt >> 3) & 15;            // pixel row of the 16-pixel k-block
-        const int half = pt >> 7;                  // group 0..2: A chunk `half` (< X_CHUNKS);  dY: taps t == half (mod 3)
-        const bool xq = half < X_CHUNKS;
+        // ---- producers: 8 warps.  Thread pt owns pixel row r = pt / 8 of every k-block and the 4-channel unit ul = pt % 8
+        //      of each 32-channel chunk: the x channels 4 ul and 32 + 4 ul, and the packed dY columns n = 32 ch + 4 ul of
+        //      every chunk with n < taps * ncol (tap n / ncol, output channel co0 + n % ncol).  A warp covers 4 pixels x 8 units.
+        const int pt = threadIdx.x - CONSUMER_THREADS;
+        const int ul = pt & 7;
+        const int row = pt >> 3;
         constexpr bool AFF = PRE >= 2;
         constexpr bool RELU = (PRE & 1) != 0;
-        // K-major core-matrix tiles: element (row n, pixel k) at (n / 8) * CORE_SBO + (k / 4) * 128 + (n % 8) * 16 + (k % 4) * 4;
-        // a thread's 4 consecutive channels of one pixel are 4 scalar stores 16 bytes apart
+        // x tile: the unit's 16 bytes go to chunk ul ^ 2 (row % 4) of the pixel's 256-byte row (chunk + 8 for the second
+        // unit).  Each 8-lane phase of a 128-bit store writes the 8 chunks of one pixel, which the XOR only permutes: no
+        // bank conflict.
+        const uint32_t xoff = (uint32_t)row * X_ROW_BYTES + ((uint32_t)(ul ^ (2 * (row & 3))) << 4);
+        // dY tiles, K-major core matrices: element (column n, pixel k) at (n / 8) * CORE_SBO + (k / 4) * 128 + (n % 8) * 16 +
+        // (k % 4) * 4, a unit = 4 scalar stores 16 bytes apart.  In 32-bit words CORE_SBO = 260 = 4 (mod 32) and a 4-pixel
+        // group is 32 words, so the bank is 4 ((n / 8) + (n % 8)) + k % 4 (mod 32).  A warp's 8 units of one chunk give
+        // (n / 8) + (n % 8) = 4 ch + ul / 2 + 4 (ul % 2) + e, 8 distinct values mod 8, and its 4 pixels distinct k % 4: each
+        // scalar store hits 32 distinct banks.
         auto core_off = [&](int n) {
             return (uint32_t)(n >> 3) * CORE_SBO + (uint32_t)(row >> 2) * 128u + (uint32_t)(n & 7) * 16u + (uint32_t)(row & 3) * 4u;
         };
         const int xs = (int)p.xs, dys = (int)p.dys;
-        const int cbx = ci_tile * BLOCK_CI + half * 32 + unit * 4;    // first x channel of this thread (chunk `half`)
-        const int cbd = co0 + unit * 4;                               // first dY channel (chunk 0)
+        const int cbx = ci_tile * BLOCK_CI + ul * 4;                  // first x channel of this thread's first unit
         const float *__restrict__ xg = p.x;
         const float *__restrict__ dg = p.dy;
-        float sc[1][4], sh[1][4];
+        float sc[2][4], sh[2][4];
         if (AFF) {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                sc[0][e] = xq ? s_scale[half * 32 + unit * 4 + e] : 0.f;
-                sh[0][e] = xq ? s_shift[half * 32 + unit * 4 + e] : 0.f;
-            }
-        }
-        // input-pixel coordinates of this thread's row, advanced by 16 pixels per k-block (no divisions in the loop)
-        int qx, qy, qb;
-        {
-            const int q = kb0 * KP + row;
-            qx = q % p.Win;
-            const int r = q / p.Win;
-            qy = r % p.Hin;
-            qb = r / p.Hin;
-        }
-        constexpr int NBU = 6;                     // dY units per thread per k-block: <= 3 taps x 2 chunks
-        constexpr int NAU = 1;                     // x units per thread per k-block
-        // Unit slots (j, ch), j = 0..2, ch = 0..1.  Multi-tap layers: tap t = half + 3j, 32-channel chunk ch of <= 2.
-        // Single-tap (1x1) layers: tap 0, chunk half + 3*(2j + ch) of <= 4 (an output tile up to 128 channels wide).
-        const bool single = taps == 1;
-        auto unit_tap = [&](int j) { return single ? 0 : half + GROUPS * j; };
-        auto unit_chunk = [&](int j, int ch) { return single ? half + GROUPS * (2 * j + ch) : ch; };
-        // tap offsets of this thread's taps, computed once: no divisions in the k-loop
-        int toy[NBU / 2], tox[NBU / 2], tky[NBU / 2];
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int j = 0; j < NBU / 2; ++j) {
-            const int t = unit_tap(j);
+                for (int e = 0; e < 4; ++e) {
+                    sc[h][e] = s_scale[h * 32 + ul * 4 + e];          // 0 beyond Cin
+                    sh[h][e] = s_shift[h * 32 + ul * 4 + e];
+                }
+        }
+        // this thread's dY units, computed once (no divisions in the k-loop): tap offsets, channel within the group,
+        // shared-memory offset in the packed tile and in a landing-ring slot
+        int toy[MAX_CHUNKS], tox[MAX_CHUNKS], ucol[MAX_CHUNKS];
+        uint32_t boff[MAX_CHUNKS], roff[MAX_CHUNKS];
+        bool blive[MAX_CHUNKS];
+#pragma unroll
+        for (int ch = 0; ch < MAX_CHUNKS; ++ch) {
+            const int n = ch * 32 + ul * 4;
+            blive[ch] = n < n_total;
+            const int t = blive[ch] ? n / ncol : 0;
             const int ky = t / p.KW, kx = t - ky * p.KW;
-            toy[j] = ky * p.dil - p.pad;
-            tox[j] = kx * p.dil - p.pad;
-            tky[j] = ky < p.KH ? ky : 0;
+            toy[ch] = ky * p.dil - p.pad;
+            tox[ch] = kx * p.dil - p.pad;
+            ucol[ch] = n - t * ncol;
+            boff[ch] = core_off(n);
+            roff[ch] = (uint32_t)ky * (uint32_t)p.seg_bytes + (uint32_t)((row + p.tox_max - tox[ch]) * p.cg + ucol[ch]) * 4u;
         }
-        // shared-memory offsets of this thread's dY units in the densely packed tile: N slot = t*ncol + channel
-        uint32_t boff[NBU];
-        bool blive[NBU];
-#pragma unroll
-        for (int j = 0; j < NBU / 2; ++j)
-#pragma unroll
-            for (int ch = 0; ch < 2; ++ch) {
-                const int t = unit_tap(j), cc = unit_chunk(j, ch);
-                const int c = unit * 4 + cc * 32;                         // channel within this CTA's group
-                const int n = t * ncol + c;
-                blive[j * 2 + ch] = t < taps && cc < nb && c < ncol;
-                boff[j * 2 + ch] = core_off(n);
-            }
+        // input-pixel coordinates of this thread's row, advanced by KP pixels per k-block (no divisions in the loop)
         struct Cursor { int qx, qy, qb; };
-        Cursor cur = {qx, qy, qb};
+        Cursor cur;
+        {
+            const int q = q_begin + row;
+            cur.qx = q % p.Win;
+            const int r = q / p.Win;
+            cur.qy = r % p.Hin;
+            cur.qb = r / p.Hin;
+        }
         auto advance = [&](Cursor &c) {
             c.qx += KP;
             while (c.qx >= p.Win) {
@@ -290,163 +282,163 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 if (++c.qy == p.Hin) { c.qy = 0; ++c.qb; }
             }
         };
-        // ---- x~ tile through the load path: this thread's pixel, channels of its chunk
-        auto load_x = [&](int it, const Cursor &c_, F4(&va)[NAU], bool &okx) {
-            const int q = (kb0 + it) * KP + row;
-            okx = q < p.Mq;
+        auto pixel_ok = [&](int it) { return q_begin + it * KP + row < q_end; };
+        // ---- x~ tile through the load path: this thread's pixel, its two 4-channel units
+        auto load_x = [&](int it, const Cursor &c_, F4(&va)[2], bool &okx) {
+            okx = pixel_ok(it);
             const int sy = UP ? (c_.qy >> 1) : c_.qy, sx = UP ? (c_.qx >> 1) : c_.qx;
-            const int xoff = ((c_.qb * p.Hs + sy) * p.Ws + sx) * xs;
+            const int xo = ((c_.qb * p.Hs + sy) * p.Ws + sx) * xs;
 #pragma unroll
-            for (int ch = 0; ch < NAU; ++ch) {
-                const int c = cbx + ch * 32;
-                const bool live = xq && okx && c < p.Cin;
+            for (int h = 0; h < 2; ++h) {
+                const int c = cbx + h * 32;
+                const bool live = okx && c < p.Cin;
                 if (VEC) {
                     float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (live) v = __ldg(reinterpret_cast<const float4 *>(xg + xoff + c));
+                    if (live) v = __ldg(reinterpret_cast<const float4 *>(xg + xo + c));
                     if (c + 3 >= p.Cin) {
                         if (c + 1 >= p.Cin) v.y = 0.f;
                         if (c + 2 >= p.Cin) v.z = 0.f;
                         v.w = 0.f;
                     }
-                    va[ch].v[0] = v.x; va[ch].v[1] = v.y; va[ch].v[2] = v.z; va[ch].v[3] = v.w;
+                    va[h].v[0] = v.x; va[h].v[1] = v.y; va[h].v[2] = v.z; va[h].v[3] = v.w;
                 } else {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
                         float v = 0.f;
-                        if (live && c + e < p.Cin) v = __ldg(xg + xoff + c + e);
-                        va[ch].v[e] = v;
+                        if (live && c + e < p.Cin) v = __ldg(xg + xo + c + e);
+                        va[h].v[e] = v;
                     }
                 }
             }
         };
-        // ---- shifted dY tiles through the load path: taps t = half, half+4, ...; output pixel (qy - dy_t, qx - dx_t)
-        auto load_d = [&](const Cursor &c_, bool okx, F4(&vb)[NBU]) {
+        // ---- shifted dY units through the load path: output pixel (qy - toy, qx - tox) of the unit's tap
+        auto load_d = [&](const Cursor &c_, bool okx, F4(&vb)[MAX_CHUNKS]) {
 #pragma unroll
-            for (int j = 0; j < NBU / 2; ++j) {
-                const int t = unit_tap(j);
-                const int py = c_.qy - toy[j], px = c_.qx - tox[j];
-                const bool okd = okx && t < taps && (unsigned)py < (unsigned)p.Hout && (unsigned)px < (unsigned)p.Wout;
+            for (int ch = 0; ch < MAX_CHUNKS; ++ch) {
+                const int py = c_.qy - toy[ch], px = c_.qx - tox[ch];
+                const bool okd = okx && blive[ch] && (unsigned)py < (unsigned)p.Hout && (unsigned)px < (unsigned)p.Wout;
                 const int doff = ((c_.qb * p.Hout + py) * p.Wout + px) * dys;
+                const int c = co0 + ucol[ch];
+                const bool live = okd && c < p.Cout;
+                F4 &dst = vb[ch];
+                if (VEC) {
+                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                    if (live) v = __ldg(reinterpret_cast<const float4 *>(dg + doff + c));
+                    if (c + 3 >= p.Cout) {
+                        if (c + 1 >= p.Cout) v.y = 0.f;
+                        if (c + 2 >= p.Cout) v.z = 0.f;
+                        v.w = 0.f;
+                    }
+                    dst.v[0] = v.x; dst.v[1] = v.y; dst.v[2] = v.z; dst.v[3] = v.w;
+                } else {
 #pragma unroll
-                for (int ch = 0; ch < 2; ++ch) {
-                    const int c = cbd + unit_chunk(j, ch) * 32;
-                    const bool live = okd && blive[j * 2 + ch] && c < p.Cout;
-                    F4 &dst = vb[j * 2 + ch];
-                    if (VEC) {
-                        float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                        if (live) v = __ldg(reinterpret_cast<const float4 *>(dg + doff + c));
-                        if (c + 3 >= p.Cout) {
-                            if (c + 1 >= p.Cout) v.y = 0.f;
-                            if (c + 2 >= p.Cout) v.z = 0.f;
-                            v.w = 0.f;
-                        }
-                        dst.v[0] = v.x; dst.v[1] = v.y; dst.v[2] = v.z; dst.v[3] = v.w;
-                    } else {
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float v = 0.f;
-                            if (live && c + e < p.Cout) v = __ldg(dg + doff + c + e);
-                            dst.v[e] = v;
-                        }
+                    for (int e = 0; e < 4; ++e) {
+                        float v = 0.f;
+                        if (live && c + e < p.Cout) v = __ldg(dg + doff + c + e);
+                        dst.v[e] = v;
                     }
                 }
             }
         };
-        auto load = [&](int it, F4(&va)[NAU], F4(&vb)[NBU], bool &okx) {
+        auto load = [&](int it, F4(&va)[2], F4(&vb)[MAX_CHUNKS], bool &okx) {
             load_x(it, cur, va, okx);
             load_d(cur, okx, vb);
             advance(cur);
         };
-        // ---- the same operands out of a landing-ring slot (TMA): raw x tile [16 px][128 ch], then KH segments [segw px][cg ch]
-        auto ring_read = [&](int it, uint32_t slot, F4(&va)[NAU], F4(&vb)[NBU], bool &okx) {
-            const int q = (kb0 + it) * KP + row;
-            okx = q < p.Mq;
+        // ---- the same operands out of a landing-ring slot (TMA): raw x tile [32 px][64 ch], then KH segments [segw px][cg ch]
+        auto ring_read = [&](int it, uint32_t slot, F4(&va)[2], F4(&vb)[MAX_CHUNKS], bool &okx) {
+            okx = pixel_ok(it);
             uint32_t segb = slot;
             if (!UP) {
-                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                if (xq) v = ld_shared_v4(slot + (uint32_t)((row * BLOCK_CI + half * 32 + unit * 4) * 4));
-                va[0].v[0] = v.x; va[0].v[1] = v.y; va[0].v[2] = v.z; va[0].v[3] = v.w;    // channels >= Cin, pixels >= Mq: zero fill
-                segb += X_RAW_BYTES;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {   // channels >= Cin and pixels >= Mq arrive as zeros (TMA zero fill)
+                    const float4 v = ld_shared_v4(slot + (uint32_t)(row * X_ROW_BYTES + (h * 32 + ul * 4) * 4));
+                    va[h].v[0] = v.x; va[h].v[1] = v.y; va[h].v[2] = v.z; va[h].v[3] = v.w;
+                }
+                segb += X_BYTES;
             }
 #pragma unroll
-            for (int j = 0; j < NBU / 2; ++j) {
-                const int t = unit_tap(j);
-                const int py = cur.qy - toy[j], px = cur.qx - tox[j];
-                const bool okd = okx && t < taps && (unsigned)py < (unsigned)p.Hout && (unsigned)px < (unsigned)p.Wout;
-                const uint32_t rowb = segb + (uint32_t)tky[j] * (uint32_t)p.seg_bytes +
-                                      (uint32_t)((row + p.tox_max - tox[j]) * p.cg + unit * 4) * 4u;
-#pragma unroll
-                for (int ch = 0; ch < 2; ++ch) {
-                    F4 &dst = vb[j * 2 + ch];
-                    float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (okd && blive[j * 2 + ch]) v = ld_shared_v4(rowb + (uint32_t)unit_chunk(j, ch) * 128u);
-                    dst.v[0] = v.x; dst.v[1] = v.y; dst.v[2] = v.z; dst.v[3] = v.w;
-                }
+            for (int ch = 0; ch < MAX_CHUNKS; ++ch) {
+                const int py = cur.qy - toy[ch], px = cur.qx - tox[ch];
+                const bool okd = okx && blive[ch] && (unsigned)py < (unsigned)p.Hout && (unsigned)px < (unsigned)p.Wout;
+                float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
+                if (okd) v = ld_shared_v4(segb + roff[ch]);
+                vb[ch].v[0] = v.x; vb[ch].v[1] = v.y; vb[ch].v[2] = v.z; vb[ch].v[3] = v.w;
             }
             advance(cur);
         };
-        auto split_store = [&](uint32_t hi_addr, uint32_t lo_addr, const F4 &v) {
-            float hi[4], lo[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) split_tf32(v.v[e], hi[e], lo[e]);
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-                st_shared_f32(hi_addr + 16u * e, hi[e]);
-                st_shared_f32(lo_addr + 16u * e, lo[e]);
-            }
-        };
         int st_s = 0;
         uint32_t st_ph = 0;
-        auto store = [&](int it, F4(&va)[NAU], F4(&vb)[NBU], bool okx) {
+        auto store = [&](F4(&va)[2], F4(&vb)[MAX_CHUNKS], bool okx) {
             const int s = st_s;
             const uint32_t ph = st_ph;
             if (++st_s == S) { st_s = 0; st_ph ^= 1; }
-            if (PRE != 0) {
 #pragma unroll
-                for (int ch = 0; ch < NAU; ++ch)
+            for (int h = 0; h < 2; ++h)
 #pragma unroll
-                    for (int e = 0; e < 4; ++e) {
-                        float a = va[ch].v[e];
-                        if (AFF) {
-                            a = fmaf(a, sc[ch][e], sh[ch][e]);
-                            if (RELU) a = fmaxf(a, 0.f);
-                            a = okx ? a : 0.f;
-                        } else {
-                            a = fmaxf(a, 0.f);
-                        }
-                        va[ch].v[e] = a;
-                    }
-            }
+                for (int e = 0; e < 4; ++e) {
+                    float a = va[h].v[e];
+                    if (AFF) a = fmaf(a, sc[h][e], sh[h][e]);
+                    if (RELU) a = fmaxf(a, 0.f);
+                    va[h].v[e] = okx ? a : 0.f;        // pixels past this CTA's range (zero padding after the pre-op)
+                }
             mbar_wait(empty(s), ph ^ 1);
-            const uint32_t a_hi = base + (uint32_t)s * (uint32_t)p.stage_bytes, a_lo = a_hi + A_BYTES;
-            const uint32_t b_hi = a_hi + 2 * A_BYTES, b_lo = b_hi + b_half;
-            if (xq) {
-                const uint32_t o = core_off(half * 32 + unit * 4);
-                split_store(a_hi + o, a_lo + o, va[0]);
-            }
+            const uint32_t st = base + (uint32_t)s * stage_bytes;
 #pragma unroll
-            for (int j = 0; j < NBU; ++j)
-                if (blive[j]) split_store(b_hi + boff[j], b_lo + boff[j], vb[j]);
-            fence_proxy_async();
+            for (int h = 0; h < 2; ++h)
+                st_shared_v4(st + xoff + 128u * h, va[h].v[0], va[h].v[1], va[h].v[2], va[h].v[3]);
+            const uint32_t b_hi = st + X_BYTES, b_lo = b_hi + (uint32_t)p.b_half;
+#pragma unroll
+            for (int ch = 0; ch < MAX_CHUNKS; ++ch) {
+                if (!blive[ch]) continue;
+                float hi[4], lo[4];
+#pragma unroll
+                for (int e = 0; e < 4; ++e) split_tf32(vb[ch].v[e], hi[e], lo[e]);
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    st_shared_f32(b_hi + boff[ch] + 16u * e, hi[e]);
+                    st_shared_f32(b_lo + boff[ch] + 16u * e, lo[e]);
+                }
+            }
+            fence_proxy_async();                       // generic-proxy dY writes -> visible to wgmma (async proxy)
             mbar_arrive(full(s));
         };
         if constexpr (!TMA) {
-            F4 a0[NAU], a1[NAU], b0[NBU], b1[NBU];
+            F4 a0[2], a1[2], b0[MAX_CHUNKS], b1[MAX_CHUNKS];
             bool k0 = false, k1 = false;
             int it = 0;
             if (it < nkb) load(it, a0, b0, k0);
             for (; it < nkb; it += 2) {
                 const bool more = it + 1 < nkb;
                 if (more) load(it + 1, a1, b1, k1);
-                store(it, a0, b0, k0);
+                store(a0, b0, k0);
                 if (more) {
                     if (it + 2 < nkb) load(it + 2, a0, b0, k0);
-                    store(it + 1, a1, b1, k1);
+                    store(a1, b1, k1);
                 }
             }
         } else {
-            // consume the landing ring; an up-sampled x still comes through the load path, one k-block ahead (own cursor)
-            F4 xc[NAU], xn[NAU], va[NAU], vb[NBU];
+            // landing ring: producer thread 0 fills slot j with k-block `it` and refills it with k-block it + ring as soon
+            // as every producer has released it.  An up-sampled x still comes through the load path, one k-block ahead.
+            auto issue = [&](int it, int j) {
+                const uint32_t dst = base + ring_off + (uint32_t)j * (uint32_t)p.slot_bytes;
+                const int q0 = q_begin + it * KP;
+                mbar_arrive_expect_tx(rfull(j), (uint32_t)p.slot_tx);
+                uint32_t seg = dst;
+                if (!UP) {
+                    tma_tile_2d(dst, &tmx, ci_tile * BLOCK_CI, q0, rfull(j));
+                    seg += X_BYTES;
+                }
+                for (int ky = 0; ky < p.KH; ++ky)     // output pixels q - (ky*dil - pad)*W - tox, tox <= tox_max
+                    tma_tile_2d(seg + (uint32_t)ky * (uint32_t)p.seg_bytes, &tmd, co0,
+                                q0 - (ky * p.dil - p.pad) * p.Wout - p.tox_max, rfull(j));
+            };
+            if (pt == 0) {
+                if (!UP) tma_prefetch_desc(&tmx);
+                tma_prefetch_desc(&tmd);
+                for (int it = 0; it < nkb && it < p.ring; ++it) issue(it, it);
+            }
+            F4 xc[2], xn[2], va[2], vb[MAX_CHUNKS];
             bool kc = false, kn = false, okx = false;
             Cursor pre = cur;
             if (UP && nkb > 0) { load_x(0, pre, xc, kc); advance(pre); }
@@ -456,15 +448,19 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 if (UP && it + 1 < nkb) { load_x(it + 1, pre, xn, kn); advance(pre); }
                 mbar_wait(rfull(rj), rph);
                 ring_read(it, base + ring_off + (uint32_t)rj * (uint32_t)p.slot_bytes, va, vb, okx);
-                mbar_arrive(rempty(rj));               // the slot's values are in registers: the loader may refill it
+                mbar_arrive(rempty(rj));               // the slot's values are in registers
+                if (pt == 0 && it + p.ring < nkb) {
+                    mbar_wait(rempty(rj), rph);
+                    issue(it + p.ring, rj);
+                }
                 if (++rj == p.ring) { rj = 0; rph ^= 1; }
                 if (UP) {
-                    store(it, xc, vb, okx);
+                    store(xc, vb, okx);
 #pragma unroll
-                    for (int ch = 0; ch < NAU; ++ch) xc[ch] = xn[ch];
+                    for (int h = 0; h < 2; ++h) xc[h] = xn[h];
                     kc = kn;
                 } else {
-                    store(it, va, vb, okx);
+                    store(va, vb, okx);
                 }
             }
         }
@@ -488,12 +484,12 @@ int bts_wgrad2_cg(int Cout, int taps) {
     return cg;
 }
 
-// used on maps of at least 12k pixels (down to the 22x44 maps of DenseNet block 3 at batch 16) with >= 8 k-blocks per
-// split-K CTA; smaller maps stay on the tap-in-grid kernel
+// used on maps of at least 12k pixels (down to the 22x44 maps of DenseNet block 3 at batch 16) with >= 8 blocks of 16
+// pixels per split-K CTA; smaller maps stay on the tap-in-grid kernel
 static long long g_w2_min_pixels = 12000;
 static int g_w2_pointwise = 1;               // 1x1 layers (64 < Cout <= 256) on this kernel too
 extern "C" int bts_wgrad2_set_pointwise(int on) { g_w2_pointwise = on ? 1 : 0; return 0; }
-static int g_w2_min_kb = 8;                  // fewest 16-pixel k-blocks a split-K CTA gets
+static int g_w2_min_kb = 8;                  // fewest 16-pixel blocks (SPLIT_PX) a split-K CTA gets
 extern "C" int bts_wgrad2_set_min_pixels(long long n) { g_w2_min_pixels = n < 0 ? 12000 : n; return 0; }
 extern "C" int bts_wgrad2_set_min_kblocks(int n) { g_w2_min_kb = n < 1 ? 8 : n; return 0; }
 
@@ -508,7 +504,7 @@ void bts_wgrad2_plan(int B, int Hin, int Win, int Cin, int Cout, int KH, int KW,
     const int taps = KH * KW;
     const int cg = bts_wgrad2_cg(Cout, taps);
     const long long Mq = (long long)B * Hin * Win;
-    const long long KBq = (Mq + KP - 1) / KP;
+    const long long KBq = (Mq + SPLIT_PX - 1) / SPLIT_PX;
     const long long tiles = (long long)((Cin + BLOCK_CI - 1) / BLOCK_CI) * ((Cout + cg - 1) / cg);
     const int sms = bts_num_sms();
     long long max_split = (KBq + g_w2_min_kb - 1) / g_w2_min_kb;
@@ -573,15 +569,14 @@ int bts_wgrad2_launch(const float *x, long long xs, int B, int Hs, int Ws, int u
     p.dy = dy; p.dys = dys; p.Cout = Cout; p.Hout = Hout; p.Wout = Wout;
     p.Hin = up ? 2 * Hs : Hs; p.Win = up ? 2 * Ws : Ws;
     p.cg = bts_wgrad2_cg(Cout, taps);
-    p.nb = (p.cg + 31) / 32;
     p.part = workspace; p.splitK = splitK;
     const long long Mq = (long long)B * p.Hin * p.Win;
     if (Mq > 0x7ffffff0LL) return BTS_EINVAL;
     p.Mq = (int)Mq;
-    p.KBq = (int)((Mq + KP - 1) / KP);
-    p.kb_per_split = (p.KBq + splitK - 1) / splitK;
-    p.nchunks = (taps * p.cg + 31) / 32;
-    p.stage_bytes = 2 * A_BYTES + 2 * p.nchunks * 4 * (int)CORE_SBO;
+    const int blocks = (int)((Mq + SPLIT_PX - 1) / SPLIT_PX);
+    p.px_per_split = (blocks + splitK - 1) / splitK * SPLIT_PX;
+    p.b_half = taps * p.cg / 8 * (int)CORE_SBO;
+    p.stage_bytes = (X_BYTES + 2 * p.b_half + 127) / 128 * 128;     // TMA ring slots that follow stay 128-byte aligned
     p.stages = SMEM_BUDGET / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     if (p.stages < 2) return BTS_EINVAL;
@@ -598,8 +593,8 @@ int bts_wgrad2_launch(const float *x, long long xs, int B, int Hs, int Ws, int u
         p.segw = KP + (KW - 1) * dil;
         p.tox_max = (KW - 1) * dil - pad;
         p.seg_bytes = (p.segw * p.cg * 4 + 127) / 128 * 128;
-        p.slot_bytes = (up ? 0 : X_RAW_BYTES) + KH * p.seg_bytes;
-        p.slot_tx = (up ? 0 : X_RAW_BYTES) + KH * p.segw * p.cg * 4;
+        p.slot_bytes = (up ? 0 : X_BYTES) + KH * p.seg_bytes;
+        p.slot_tx = (up ? 0 : X_BYTES) + KH * p.segw * p.cg * 4;
         int st_try = p.stages > 3 ? 3 : p.stages;
         for (; st_try >= 2 && !tma; --st_try) {
             const int ring = (SMEM_BUDGET - st_try * p.stage_bytes) / p.slot_bytes;
