@@ -10,9 +10,10 @@
 //              (upconv, bts.py:77) which is folded into the address map -- the 4x tensor is never materialised.
 //       act  = none | ELU | sigmoid, fused in the epilogue.
 //
-// GEMM view: M = B*Hout*Wout pixels (128 per CTA tile: two warpgroups of 64 rows), N = Cout (<= 64 per tile: the
-// k-block accumulator and the tile sum of a 64 x 64 tile are 64 registers per thread), K = the dense sequence of 16-byte channel quads,
-// tap-major, in blocks of 32 fp32 (one 128-byte swizzled row per pixel).
+// GEMM view: M = B*Hout*Wout pixels (128 per CTA tile: two warpgroups of 64 rows), N = Cout (<= 128 per tile, equal
+// tiles in multiples of 16: the k-block accumulator and the tile sum of a 64 x 128 warpgroup tile are 128 registers per
+// thread), K = the dense sequence of 16-byte channel quads, tap-major, in blocks of 32 fp32 (one 128-byte swizzled row per
+// pixel).
 // Precision: fp32 operands are split x = hi + lo with hi = x rounded to tf32, lo = x - hi and the tile accumulates
 // A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with tf32 wgmma into fp32 register accumulators (error ~2^-21 per product:
 // fp32-grade, SURVEY Appendix F); every k-block's tensor-core sum is added into the tile sum with round-to-nearest fp32
@@ -22,16 +23,18 @@
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... with the smem stage
 // ring and all warp roles running continuously across tile boundaries (the producers fill the stages of tile t+1 while
 // the consumers run the epilogue of tile t; no per-tile launch or pipeline-fill cost).
-// Warp roles (512 threads = 16 warps, 128 registers per thread, 1 CTA/SM):
+// Warp roles (512 threads = 16 warps launched with 128 registers per thread, 1 CTA/SM; setmaxnreg then moves registers
+// from the producers, which keep 80, to the consumers, which get 176):
 //   warps 0..7  : two consumer warpgroups -- per k-block, each thread loads its A fragments (fp32) from the swizzled tile,
 //                 splits them into hi/lo in registers and issues register-A wgmma against the B hi/lo tiles in shared
 //                 memory; then the epilogue from the accumulator registers: activation, NHWC stores, optional BatchNorm
 //                 batch statistics of the output;
 //   warps 8..15 : two producer groups (alternating k-blocks).  One lane of the group filling a k-block streams its
 //                 pre-packed, pre-split, pre-swizzled weight tile with a 1-D bulk async copy (cp.async.bulk) completing on
-//                 the stage's mbarrier (in TMA mode also the im2col activation tile); the group's threads make coalesced
-//                 128-bit global loads of the activation tile (8 lanes cover one pixel's 128 B), apply the pre-op in
-//                 registers, one swizzled 128-bit shared store per (row, chunk), fence.proxy.async, mbarrier arrive.
+//                 the stage's mbarrier (in TMA mode also the im2col activation tile); the group's threads copy the
+//                 activation tile from global memory straight into its swizzled slots with 16-byte cp.async (8 lanes cover
+//                 one pixel's 128 B; padding is zero-filled), whose completion is their arrival on the stage's mbarrier;
+//                 with a BatchNorm / ReLU pre-op they wait for the copies and apply it in place first.
 // Staging A as fp32 and splitting it in the consumers keeps shared-memory traffic per k-block at one A tile written and
 // read once (A from shared memory through descriptors would be read by each of the three products).
 #include <cstdio>
@@ -47,11 +50,17 @@ namespace {
 
 constexpr int BLOCK_M = 128;
 constexpr int BLOCK_K = 32;                 // fp32 elements per k-block = one 128-byte row
-constexpr int MAX_N = 64;                   // output channels per tile (two register accumulators per consumer thread)
+constexpr int MAX_N = 128;                  // output channels per tile (two register accumulators per consumer thread)
 constexpr int A_TILE_BYTES = BLOCK_M * 128; // 16 KB of fp32 activations
 constexpr int CONSUMER_THREADS = 256;       // two warpgroups
 constexpr int PRODUCER_THREADS = 128;       // per group
 constexpr int NUM_THREADS = CONSUMER_THREADS + 2 * PRODUCER_THREADS;   // 16 warps: 128 registers per thread
+// registers per thread after the warpgroups' reallocation (setmaxnreg): the producers hand theirs to the consumers, whose
+// k-block accumulator, tile sum and A fragments are 64 + 64 + 32 registers at N = 128
+constexpr int PRODUCER_REGS = 80;
+constexpr int CONSUMER_REGS = 176;
+static_assert(CONSUMER_THREADS * CONSUMER_REGS + 2 * PRODUCER_THREADS * PRODUCER_REGS <= NUM_THREADS * 128,
+              "the reallocation must fit the registers the CTA was launched with");
 constexpr int MAX_CIN_SMEM = 4096;          // pre-op scale/shift staged in smem (32 KB at most)
 
 struct ConvParams {
@@ -266,6 +275,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
 
     if (threadIdx.x >= CONSUMER_THREADS) {
         // ===================== producers (two groups x 4 warps, alternating k-blocks) =====================
+        setmaxnreg_dec<PRODUCER_REGS>();
         // The group that fills a k-block also stages its weight tile: right after the stage has been released, one lane
         // issues the 1-D bulk async copy (cp.async.bulk) of the pre-packed, pre-split, pre-swizzled B hi/lo rows -- and,
         // in TMA mode, the im2col load of the activation tile -- completing on an mbarrier.
@@ -383,10 +393,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
                 while (kb >= KB) { kb -= KB; ++ti; }
             }
         } else {
-        // ---- LOAD cursor: (tile iteration, k-block in tile) of the next k-block this group loads; this lane's channel
-        //      quad of that k-block is g = 8 kb + chunk -> (tap, quad in tap) by multiply-shift division
-        // oyx[i]: the row's top-left source coordinate, (oy << 16) | (ox & 0xffff) -- one register per row instead of two,
-        // so that a k-block of loads in flight and one being stored fit the register budget (host: |coordinates| < 2^14)
+        // ---- cursor: (tile iteration, k-block in tile) of the next k-block this group fills; this lane's channel quad of
+        //      that k-block is g = 8 kb + chunk -> (tap, quad in tap) by multiply-shift division
+        // oyx[i]: the row's top-left source coordinate, (oy << 16) | (ox & 0xffff) -- one register per row instead of two
+        // (host: |coordinates| < 2^14)
         int oyx[8], rowoff[8];
         int l_ti = 0, l_kb = grp, cur_ti = -1, cur_nt = 0;      // (KB may be 1)
         while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
@@ -415,11 +425,56 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
                 }
             }
         };
-        // ---- load phase: this lane's 8 x 16-byte global loads of one k-block (predicated, branch-free); w_out = index of
-        //      the k-block's weight tile in wpack (n-tile * KB + kb; host guarantees < 2^31)
-        auto load_kb = [&](F4(&v)[8], uint32_t &mask, int &c_out, int &w_out) {
+        // ---- pre-op of a landed k-block, in place (this thread's own 8 slots): BatchNorm-apply and/or ReLU; rows in the
+        //      padding (mask bit clear) are re-zeroed, because the padding is applied after the pre-op
+        auto pre_op = [&](const uint32_t a_st, const uint32_t mask, const int c) {
+            float sc[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
+            if (AFF) {
+                const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
+                const float4 b4 = *reinterpret_cast<const float4 *>(s_shift + c);
+                sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
+                sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
+            }
+#pragma unroll
+            for (int i = 0; i < 8; ++i) {
+                const float4 q4 = ld_shared_v4(a_st + (uint32_t)i * 2048u);
+                float v[4] = {q4.x, q4.y, q4.z, q4.w};
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    float a = v[e];
+                    if (AFF) {
+                        a = fmaf(a, sc[e], sh[e]);              // scale/shift are 0 beyond Cin
+                        if (RELU) a = fmaxf(a, 0.f);
+                        a = ((mask >> i) & 1u) ? a : 0.f;
+                    } else if (RELU) {
+                        a = fmaxf(a, 0.f);                      // padded rows landed as zeros
+                    }
+                    v[e] = a;
+                }
+                st_shared_v4(a_st + (uint32_t)i * 2048u, v[0], v[1], v[2], v[3]);
+            }
+        };
+        // ---- per k-block: wait for the stage, stage its weights, then one asynchronous copy (cp.async, LDGSTS) per
+        //      (row, chunk) from global memory straight into the row's swizzled slot.  Padding, rows past M, quads past
+        //      the last tap and the odd coordinates of the zero-stuffed source copy 0 bytes (zero-filled); the Cin % 4
+        //      tail copies the live channels only.  Without a pre-op the copies' completion is the thread's arrival on
+        //      the stage's full barrier, so a producer never waits for its own loads and runs ahead as far as the ring
+        //      allows.  With a pre-op the thread waits for the copies of its PREVIOUS k-block (one k-block of copies
+        //      stays in flight; needs S >= 3, else it waits for the current one), transforms them in place and arrives.
+        int s_s = grp;                             // stage of this group's next k-block (S >= 2)
+        uint32_t s_ph = 0;
+        int pend_s = -1;                           // pre-op: stage of the k-block whose copies are in flight (-1: none)
+        uint32_t pend_mask = 0;
+        int pend_c = 0;
+        auto publish_pending = [&]() {
+            pre_op(base + (uint32_t)pend_s * stage_bytes + roff0, pend_mask, pend_c);
+            mbar_arrive(full(pend_s));
+        };
+        const int mine = total_kb > grp ? (total_kb - grp + 1) / 2 : 0;   // k-blocks of this group
+#pragma unroll 1
+        for (int it = 0; it < mine; ++it) {
             if (l_ti != cur_ti) set_tile(l_ti);
-            w_out = cur_nt * KB + l_kb;
+            const int w = cur_nt * KB + l_kb;      // the k-block's weight tile in wpack (host guarantees < 2^31)
             uint32_t g = (uint32_t)(l_kb * 8 + chunk);
             uint32_t tap = fdiv(g, p.fd_cq);
             if (p.chunk_major) {                   // (chunk, tap) order: one tap per k-block, the chunk advances every `taps` k-blocks
@@ -432,8 +487,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
             const int dy = (int)ky * dil, dx = kx * dil;
             const bool cok = (int)tap < taps;      // quads past the last tap pad the final k-block
             const int c = cok ? (int)(g - tap * (uint32_t)p.CQ) * 4 : 0;   // first channel of this lane's 16-byte unit
-            c_out = c;
             const int tapoff = UP ? c : (dy * Ws + dx) * xs + c;
+            const uint32_t vbytes = c + 4 <= Cin ? 16u : (uint32_t)(Cin - c) * 4u;
+            const uint32_t stage = base + (uint32_t)s_s * stage_bytes;
+            const uint32_t a_st = stage + roff0;
+            const uint32_t bar_full = full(s_s);
+            mbar_wait(empty(s_s), s_ph ^ 1);
+            if (issuer) {
+                mbar_arrive_expect_tx(bar_full, wbytes);
+                bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + (size_t)w * wbytes, wbytes, bar_full);
+            }
             uint32_t mk = 0;
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -444,91 +507,45 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
                 int off;
                 if (UP) off = rowoff[i] + ((yy >> 1) * Ws + (xx >> 1)) * xs + tapoff;
                 else off = rowoff[i] + tapoff;
+                const uint32_t dst = a_st + (uint32_t)i * 2048u;
                 if (VEC) {
-                    float4 q = make_float4(0.f, 0.f, 0.f, 0.f);
-                    if (ok) q = __ldg(reinterpret_cast<const float4 *>(xg + off));
-                    v[i].v[0] = q.x; v[i].v[1] = q.y; v[i].v[2] = q.z; v[i].v[3] = q.w;
+                    cp_async16(dst, ok ? xg + off : xg, ok ? vbytes : 0u);
                 } else {
 #pragma unroll
                     for (int e = 0; e < 4; ++e) {
-                        float q = 0.f;
-                        if (ok && c + e < Cin) q = __ldg(xg + off + e);
-                        v[i].v[e] = q;
+                        const bool oke = ok && c + e < Cin;
+                        cp_async4(dst + 4u * e, oke ? xg + off + e : xg, oke ? 4u : 0u);
                     }
                 }
             }
-            mask = mk;
-            l_kb += 2;
-            while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
-        };
-        // ---- store phase: wait for the stage, stage its weights, pre-op in registers, swizzled 128-bit stores, publish
-        int s_s = grp;                             // stage of this group's next store (S >= 2)
-        uint32_t s_ph = 0;
-        auto store_kb = [&](F4(&v)[8], uint32_t mask, const int c, const int w) {
-            const uint32_t stage = base + (uint32_t)s_s * stage_bytes;
-            const uint32_t a_st = stage + roff0;
-            const uint32_t bar_full = full(s_s);
-            mbar_wait(empty(s_s), s_ph ^ 1);
-            if (issuer) {
-                mbar_arrive_expect_tx(bar_full, wbytes);
-                bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + (size_t)w * wbytes, wbytes, bar_full);
+            if constexpr (PRE == 0) {
+                cp_async_mbar_arrive(bar_full);
+            } else {
+                cp_async_commit();
+                if (pend_s >= 0) {
+                    cp_async_wait_dyn(1);
+                    publish_pending();
+                }
+                pend_s = s_s; pend_mask = mk; pend_c = c;
+                if (S < 3) {                       // the group's next stage may be the one still waiting to be published
+                    cp_async_wait_dyn(0);
+                    publish_pending();
+                    pend_s = -1;
+                }
             }
             s_s += 2;
             if (s_s >= S) { s_s -= S; s_ph ^= 1; }
-            float sc[4], sh[4];
-            if (AFF) {
-                const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
-                const float4 b4 = *reinterpret_cast<const float4 *>(s_shift + c);
-                sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
-                sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
-            }
-            if (VEC && c < Cin && c + 3 >= Cin) {
-                // channel tail (Cin % 4 != 0, rows padded to 16 B): the float4 read past Cin -- zero those lanes
-#pragma unroll
-                for (int i = 0; i < 8; ++i)
-#pragma unroll
-                    for (int e = 1; e < 4; ++e)
-                        if (c + e >= Cin) v[i].v[e] = 0.f;
-            }
-#pragma unroll
-            for (int i = 0; i < 8; ++i) {
-                const bool live = (mask >> i) & 1u;
-                float a[4];
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    a[e] = v[i].v[e];
-                    if (AFF) {
-                        a[e] = fmaf(a[e], sc[e], sh[e]);        // scale/shift are 0 beyond Cin
-                        if (RELU) a[e] = fmaxf(a[e], 0.f);
-                        a[e] = live ? a[e] : 0.f;               // zero padding is applied after the pre-op
-                    } else if (RELU) {
-                        a[e] = fmaxf(a[e], 0.f);                // padded lanes were loaded as 0
-                    }
-                }
-                st_shared_v4(a_st + (uint32_t)i * 2048u, a[0], a[1], a[2], a[3]);
-            }
-            fence_proxy_async();               // generic-proxy writes -> visible to the tensor-core (async) proxy
-            mbar_arrive(bar_full);
-        };
-        // ---- software pipeline (register ping-pong): the loads of this group's next k-block -- possibly of the next
-        //      tile -- are in flight while the current one is transformed and stored
-        const int mine = total_kb > grp ? (total_kb - grp + 1) / 2 : 0;   // k-blocks of this group
-        F4 va[8], vb[8];
-        uint32_t ma = 0, mb = 0;
-        int ca = 0, cb = 0, wa = 0, wb = 0;
-        int issued = 0;
-        if (issued < mine) { load_kb(va, ma, ca, wa); ++issued; }
-        for (int done = 0; done < mine; done += 2) {
-            if (issued < mine) { load_kb(vb, mb, cb, wb); ++issued; }
-            store_kb(va, ma, ca, wa);
-            if (done + 1 < mine) {
-                if (issued < mine) { load_kb(va, ma, ca, wa); ++issued; }
-                store_kb(vb, mb, cb, wb);
-            }
+            l_kb += 2;
+            while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
+        }
+        if (PRE != 0 && pend_s >= 0) {
+            cp_async_wait_dyn(0);
+            publish_pending();
         }
         }   // !TMA
     } else {
         // ===================== consumers: two warpgroups, rows [64 wg, 64 wg + 64) of every 128-pixel tile =========
+        setmaxnreg_inc<CONSUMER_REGS>();
         // 3xTF32: every thread loads its A fragments of the k-block from the swizzled fp32 tile and splits them in
         // registers: hi = x rounded to tf32 (round-half-away on the 13 dropped bits, 2 integer ops), lo = x - hi, exact in
         // fp32 (the tensor core reads its top 19 bits: error <= 2^-21 |x|).  (Truncating instead of rounding saves one op
@@ -563,7 +580,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
 #pragma unroll
                 for (int i = 0; i < R; ++i) tot[i] = 0.f;
                 for (int kb = 0; kb < KB; ++kb) {
-                    mbar_wait(full(s), ph);
+                    mbar_wait_no_trap(full(s), ph);
                     uint32_t hi[BLOCK_K / 8][4], lo[BLOCK_K / 8][4];
 #pragma unroll
                     for (int k = 0; k < BLOCK_K / 8; ++k) {
@@ -711,7 +728,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
             case 16: consume(std::integral_constant<int, 16>()); break;
             case 32: consume(std::integral_constant<int, 32>()); break;
             case 48: consume(std::integral_constant<int, 48>()); break;
-            default: consume(std::integral_constant<int, 64>()); break;
+            case 64: consume(std::integral_constant<int, 64>()); break;
+            case 80: consume(std::integral_constant<int, 80>()); break;
+            case 96: consume(std::integral_constant<int, 96>()); break;
+            case 112: consume(std::integral_constant<int, 112>()); break;
+            default: consume(std::integral_constant<int, 128>()); break;
         }
         if (p.stat_sum && p.n_tiles == 1) {
             asm volatile("bar.sync 1, %0;" ::"n"(CONSUMER_THREADS) : "memory");

@@ -31,6 +31,24 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
         if (++spins > 200000000u) __trap();   // watchdog: a protocol bug must fail loudly, not hang the box
     }
 }
+// The same wait for warps that have grown their registers with setmaxnreg.inc: a trap anywhere in such a region makes
+// ptxas hold the region to the launch-time register count (it spills instead), so on expiry the watchdog ends the thread.
+// The stages such a thread no longer releases then stall the warps that refill them, whose own waits trap.
+__device__ __forceinline__ void mbar_wait_no_trap(uint32_t bar, uint32_t parity) {
+    uint32_t ok = 0;
+    uint32_t spins = 0;
+    while (true) {
+        asm volatile(
+            "{\n\t.reg .pred p;\n\t"
+            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+            "selp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(ok)
+            : "r"(bar), "r"(parity)
+            : "memory");
+        if (ok) break;
+        if (++spins > 200000000u) asm volatile("exit;");
+    }
+}
 __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void *src, uint32_t bytes, uint32_t bar) {
     asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                  "l"(src), "r"(bytes), "r"(bar)
@@ -90,6 +108,13 @@ __device__ __forceinline__ uint64_t make_desc_core(uint32_t saddr, uint32_t lbo,
            ((uint64_t)((sbo >> 4) & 0x3FFFu) << 32);
 }
 
+// warpgroup register reallocation (setmaxnreg): all warps of a warpgroup execute it; the CTA's register pool is fixed
+// at launch, so the warpgroups that shrink must do so for the ones that grow to get their registers
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R)); }
+
 __device__ __forceinline__ float rna_tf32(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
@@ -137,6 +162,11 @@ __device__ __forceinline__ void cp_async4(uint32_t dst, const void *src, uint32_
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+// one arrival on the mbarrier once every cp.async this thread has issued so far has landed (counted in the barrier's
+// expected arrivals: .noinc)
+__device__ __forceinline__ void cp_async_mbar_arrive(uint32_t bar) {
+    asm volatile("cp.async.mbarrier.arrive.noinc.shared::cta.b64 [%0];" ::"r"(bar) : "memory");
+}
 __device__ __forceinline__ void cp_async_wait_dyn(int pending) {   // wait until <= pending groups are in flight
     switch (pending) {
         case 0: asm volatile("cp.async.wait_group 0;" ::: "memory"); break;
