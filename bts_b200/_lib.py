@@ -75,21 +75,18 @@ SIGNATURES = {
     "bts_plane_head_bwd": [_p, _p, _p, _p, _f, _i, _i, _i, _i, _i, _p],
     "bts_conv_n_tile": [_i],
     "bts_conv_packed_floats": [_i, _i, _i, _i],
-    "bts_conv_pack_weights": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _i, _p, _p],
+    "bts_conv_pack_weights": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _p, _p],
     "bts_conv_fwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p],
     "bts_conv_fwd_stats": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p, _p, _p],
     "bts_conv_fwd_ex": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p,
-                        _p, _i, _p],
+                        _p, _p],
     "bts_conv_fwd_bnbwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _ll, _i, _p, _ll, _p, _i,
-                           _p, _p, _i, _p],
+                           _p, _p, _p],
     "bts_bn_bwd_coef": [_p, _p, _ll, _i, _p, _p, _p, _p, _p],
-    "bts_conv_set_tma": [_i],
-    "bts_conv_get_tma": [],
-    "bts_conv_set_producer_groups": [_i],
     "bts_conv_group_window": [_i, _i],
     "bts_conv_packed_floats_grouped": [_i, _i, _i, _i],
     "bts_conv_group_n_tile": [_i],
-    "bts_conv_pack_weights_grouped": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _i, _p, _p],
+    "bts_conv_pack_weights_grouped": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _p, _p],
     "bts_conv_wgrad_grouped_plan": [_i, _i, _i, _i, _i, _i, _i, _p, _p],
     "bts_conv_wgrad_grouped": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _ll, _p, _i, _p, _ll, _ll, _ll, _ll, _i, _p],
     "bts_conv_wgrad_plan": [_i, _i, _i, _i, _i, _i, _i, _i, _p, _p],

@@ -63,9 +63,6 @@ def trace_report():
     return sorted(((t, n, k, f) for k, (t, n, f) in agg.items()), reverse=True)
 
 
-if _os.environ.get("BTS_B200_TMA") is not None:            # bring-up switch for the TMA-staged activation tiles
-    _lib.lib().bts_conv_set_tma(int(_os.environ["BTS_B200_TMA"]))
-
 if _os.environ.get("BTS_B200_W2_TMA") is not None:         # 0: narrow-output wgrad producers load from global memory
     _lib.lib().bts_wgrad2_set_tma(int(_os.environ["BTS_B200_W2_TMA"]))
 
@@ -100,7 +97,7 @@ def repack_cached():
         assert dt.itemsize == 96
         tab = np.zeros(len(live), dtype=dt)
         start = 0
-        for i, ((wid, tf, fl), (ref, ver, ptr, packed, groups)) in enumerate(live):
+        for i, ((wid, tf), (ref, ver, ptr, packed, groups)) in enumerate(live):
             w = ref()
             Cout, Cin, KH, KW = w.shape
             st = w.stride()
@@ -113,7 +110,7 @@ def repack_cached():
                 n_tile = L.bts_conv_n_tile(rows)
                 n_tiles, kwin, cpg, ci_tot = (rows + n_tile - 1) // n_tile, 0, 1, Cin
             tab[i] = (w.data_ptr(), packed.data_ptr(), st[0], st[1], st[2], st[3], start, Cout, ci_tot, KH, KW, int(tf),
-                      n_tile, n_tiles, kwin, cpg, int(fl))
+                      n_tile, n_tiles, kwin, cpg, 0)
             start += packed.numel() // 2
         dev = live[0][1][3].device
         _multi_plan = (sig, torch.from_numpy(tab.view(np.uint8)).to(dev), start, dev)
@@ -131,27 +128,10 @@ def group_window(width, cpg):
     return _lib.lib().bts_conv_group_window(int(width), int(cpg))
 
 
-CHUNK_MAJOR = _os.environ.get("BTS_B200_CHUNK_MAJOR", "0") == "1"
-
-
-def pack_flags(weight_shape, transpose_flip=False, groups=1):
-    """packing / kernel flags of a layer.  bit 0 = chunk-major K order: for multi-tap kernels whose K channels are whole
-    32-channel chunks, k-blocks run (chunk, tap) with the taps innermost, so the nine shifted reads of a pixel's channel chunk
-    are consecutive and hit in L1.  It is off by default: the narrow layers it targets are bound by operand staging, not L2
-    (BTS_B200_CHUNK_MAJOR=1 enables it; tests/test_conv_order_gpu.py keeps it correct)."""
-    Cout, Cin, KH, KW = weight_shape
-    if not CHUNK_MAJOR or KH * KW == 1:
-        return 0
-    kch = group_window(Cout, Cin) if groups > 1 else (Cout if transpose_flip else Cin)
-    return 1 if kch and kch % 32 == 0 else 0
-
-
-def pack_weights(weight, transpose_flip=False, groups=1, flags=None):
+def pack_weights(weight, transpose_flip=False, groups=1):
     """(Cout,Cin/groups,KH,KW) fp32 parameter -> packed operator.  Cached on the tensor's version counter."""
     _need_cuda(weight)
-    if flags is None:
-        flags = pack_flags(weight.shape, transpose_flip, groups)
-    key = (id(weight), bool(transpose_flip), int(flags))
+    key = (id(weight), bool(transpose_flip))
     ent = _pack_cache.get(key)
     w = weight.detach()
     if ent is not None:
@@ -168,13 +148,13 @@ def pack_weights(weight, transpose_flip=False, groups=1, flags=None):
         packed = torch.empty(L.bts_conv_packed_floats_grouped(Cout, Cin, KH, KW), device=w.device, dtype=torch.float32)
         with torch.cuda.device(w.device):
             _lib.check(L.bts_conv_pack_weights_grouped(_ptr(w), s[0], s[1], s[2], s[3], Cout, Cin, KH, KW,
-                                                       int(transpose_flip), int(flags), _ptr(packed), _stream()),
+                                                       int(transpose_flip), _ptr(packed), _stream()),
                        "bts_conv_pack_weights_grouped")
     else:
         packed = torch.empty(L.bts_conv_packed_floats(rows, kch, KH, KW), device=w.device, dtype=torch.float32)
         with torch.cuda.device(w.device):
             _lib.check(L.bts_conv_pack_weights(_ptr(w), s[0], s[1], s[2], s[3], Cout, Cin, KH, KW, int(transpose_flip),
-                                               int(flags), _ptr(packed), _stream()), "bts_conv_pack_weights")
+                                               _ptr(packed), _stream()), "bts_conv_pack_weights")
     _lib.count()
     _pack_cache[key] = (weakref.ref(weight), weight._version, w.data_ptr(), packed, int(groups))
     if len(_pack_cache) > 4096:
@@ -249,11 +229,8 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         _lib.check(rc, "bts_conv_pw_fwd")
         _lib.count()
         return out
-    flags = pack_flags(weight.shape, transpose_flip, groups)
-    if upsample2 or zero_stuff_out is not None:
-        flags &= ~1                          # the up-sampled / zero-stuffed address maps keep the dense tap-major K order
     if packed is None:
-        packed = pack_weights(weight, transpose_flip, groups, flags)
+        packed = pack_weights(weight, transpose_flip, groups)
     if zero_stuff_out is not None:
         mode = 2
         Hout, Wout = int(zero_stuff_out[0]), int(zero_stuff_out[1])
@@ -292,7 +269,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
                                                                Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding,
                                                                dilation, _ptr(packed), Co, _ptr(out), os_, int(precision),
                                                                _ptr(xb), xbs, _ptr(st), int(bool(relu)), _ptr(stats[0]),
-                                                               _ptr(stats[1]), int(flags), _stream()),
+                                                               _ptr(stats[1]), _stream()),
                          2.0 * B * Hout * Wout * Co * (Cin // groups) * KH * KW)
         _lib.check(rc, "bts_conv_fwd_bnbwd")
         _lib.count()
@@ -303,7 +280,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
                                                   _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift), int(pre_relu),
                                                   _ptr(out), os_, ACT[act], int(precision),
                                                   _ptr(stats[0]) if stats is not None else None,
-                                                  _ptr(stats[1]) if stats is not None else None, int(flags), _stream())
+                                                  _ptr(stats[1]) if stats is not None else None, _stream())
         rc = _traced("dgrad" if transpose_flip else "fwd",
                      "%dx%dx%d %d->%d k%d d%d s%d%s%s" % (B, Hs, Ws, Cin, Co, KH, dilation, stride,
                                                          " up" if upsample2 else (" zs" if mode == 2 else ""),

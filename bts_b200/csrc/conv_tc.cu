@@ -31,18 +31,15 @@
 //                 batch statistics of the output;
 //   warps 8..15 : two producer groups (alternating k-blocks).  One lane of the group filling a k-block streams its
 //                 pre-packed, pre-split, pre-swizzled weight tile with a 1-D bulk async copy (cp.async.bulk) completing on
-//                 the stage's mbarrier (in TMA mode also the im2col activation tile); the group's threads copy the
-//                 activation tile from global memory straight into its swizzled slots with 16-byte cp.async (8 lanes cover
-//                 one pixel's 128 B; padding is zero-filled), whose completion is their arrival on the stage's mbarrier;
-//                 with a BatchNorm / ReLU pre-op they wait for the copies and apply it in place first.
+//                 the stage's mbarrier; the group's threads copy the activation tile from global memory straight into its
+//                 swizzled slots with 16-byte cp.async (8 lanes cover one pixel's 128 B; padding is zero-filled), whose
+//                 completion is their arrival on the stage's mbarrier; with a BatchNorm / ReLU pre-op they wait for the
+//                 copies and apply it in place first.
 // Staging A as fp32 and splitting it in the consumers keeps shared-memory traffic per k-block at one A tile written and
 // read once (A from shared memory through descriptors would be read by each of the three products).
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <type_traits>
-
-#include <cuda.h>
 
 #include "tc_common.cuh"
 
@@ -87,18 +84,13 @@ struct ConvParams {
     int vec_ok;              // 16-byte aligned rows -> float4 loads
     long long M;             // B*Hout*Wout
     int m_tiles, total_tiles;
-    int KC;                  // ceil(Cin/32)
+    int KC;                  // ceil(Cin/32): 32-channel chunks of the pre-op scale/shift staged in smem
     int CQ;                  // ceil(Cin/4): 16-byte channel quads per tap (dense-K order, see the pack kernel)
     int KB;                  // ceil(KH*KW*CQ / 8) k-blocks
     tc::FastDiv fd_cq, fd_kw;
     double *stat_sum, *stat_sumsq;   // optional per-output-channel sum / sum of squares of the (activated) output
     // BatchNorm-backward reduction fused into a dgrad's epilogue (bnb_x != null): the tile being written is g = dL/d relu(bn(x));
     // stat_sum[c] += sum_p g*[bn(x)>0],  stat_sumsq[c] += sum_p g*[bn(x)>0]*xhat   (bts_bn_relu_bwd_reduce without its pass)
-    int chunk_major;         // K order: k-block kb = (chunk kb / taps, tap kb % taps) -- consecutive k-blocks re-read the SAME
-                             // pixels' lines shifted by one tap, so they hit in L1 instead of going to L2 nine times
-    int tma_adj;             // TMA mode: base-pixel coordinate = out*stride - tma_adj (the bounding box's lower corner)
-    tc::FastDiv fd_taps;     // chunk-major: kb -> (kb / taps, kb % taps)
-    tc::FastDiv fd_kc;       // TMA mode: k-block -> (tap, 32-channel chunk) = (kb / KC, kb % KC)
     const float *bnb_x; long long bnb_xs;
     const float *bnb_st;             // [4][Cout]: scale, shift, mean, invstd
     int bnb_relu;
@@ -119,8 +111,7 @@ using namespace tc;
 // transpose_flip=1 packs the dgrad operator: rows = ci, k = (flipped tap, co).
 __device__ __forceinline__ void pack_one(const float *__restrict__ w, long long s_co, long long s_ci, long long s_kh,
                                          long long s_kw, int Cout, int Cin, int KH, int KW, int transpose_flip,
-                                         float *__restrict__ wpack, int n_tile, int kwin, int cpg, int flags,
-                                         long long idx) {
+                                         float *__restrict__ wpack, int n_tile, int kwin, int cpg, long long idx) {
     // grouped (kwin > 0): Cin == Cout == total width, w is (width, cpg, KH, KW); rows = all channels, the K channels of
     // n-tile nt are the window of kwin channels that holds its rows (n_tile divides kwin) and entries outside the row's
     // group are zero (block diagonal)
@@ -136,12 +127,8 @@ __device__ __forceinline__ void pack_one(const float *__restrict__ w, long long 
     const int kb = (int)(t % KB);
     const int nt = (int)(t / KB);
     const int g = kb * 8 + (kk >> 2);
-    int tap = g / CQ;
-    int ch = (g - tap * CQ) * 4 + (kk & 3);
-    if (flags & 1) {                      // chunk-major K order (Kch % 32 == 0): k-block = (32-channel chunk, tap), taps innermost
-        tap = kb % taps;
-        ch = (kb / taps) * 32 + kk;
-    }
+    const int tap = g / CQ;
+    const int ch = (g - tap * CQ) * 4 + (kk & 3);
     const int row = nt * n_tile + n;
     float val = 0.f;
     if (row < Nrows && tap < taps && ch < Kch) {
@@ -174,13 +161,13 @@ __device__ __forceinline__ void pack_one(const float *__restrict__ w, long long 
 __global__ void __launch_bounds__(256) pack_weights_kernel(const float *__restrict__ w, long long s_co, long long s_ci,
                                                            long long s_kh, long long s_kw, int Cout, int Cin, int KH,
                                                            int KW, int transpose_flip, float *__restrict__ wpack,
-                                                           int n_tile, int n_tiles, int kwin, int cpg, int flags) {
+                                                           int n_tile, int n_tiles, int kwin, int cpg) {
     const int Kch = kwin ? kwin : (transpose_flip ? Cout : Cin);
     const int KB = (KH * KW * ((Kch + 3) / 4) + 7) / 8;
     const long long total = (long long)n_tiles * KB * n_tile * 32;
     for (long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x; idx < total;
          idx += (long long)gridDim.x * blockDim.x)
-        pack_one(w, s_co, s_ci, s_kh, s_kw, Cout, Cin, KH, KW, transpose_flip, wpack, n_tile, kwin, cpg, flags, idx);
+        pack_one(w, s_co, s_ci, s_kh, s_kw, Cout, Cin, KH, KW, transpose_flip, wpack, n_tile, kwin, cpg, idx);
 }
 
 // every packed operator of a model in ONE launch (after an optimizer step: 394 launches -> 1 for DenseNet-161 + decoder)
@@ -189,7 +176,8 @@ struct PackDesc {
     float *wpack;
     long long s_co, s_ci, s_kh, s_kw;
     long long start;                     // first global index of this operator (prefix sum of packed_floats / 2)
-    int Cout, Cin, KH, KW, transpose_flip, n_tile, n_tiles, kwin, cpg, flags;   // flags bit 0: chunk-major K order
+    int Cout, Cin, KH, KW, transpose_flip, n_tile, n_tiles, kwin, cpg;
+    int pad_;                            // explicit padding (written as 0)
 };
 static_assert(sizeof(PackDesc) == 96, "PackDesc layout is mirrored by bts_b200/conv.py");
 
@@ -203,7 +191,7 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackDesc 
         }
         const PackDesc &q = d[lo];
         pack_one(q.w, q.s_co, q.s_ci, q.s_kh, q.s_kw, q.Cout, q.Cin, q.KH, q.KW, q.transpose_flip, q.wpack, q.n_tile, q.kwin,
-                 q.cpg, q.flags, idx - q.start);
+                 q.cpg, idx - q.start);
     }
 }
 
@@ -223,13 +211,8 @@ constexpr int STAT_SETS = CONSUMER_THREADS / 32;
 //
 // Index arithmetic: every k-block -> (tile, tap, channel chunk, stage, phase) mapping is carried in incrementally updated
 // counters, and the per-tile pixel decode uses multiply-shift division by host-precomputed constants (FastDiv).
-// TMA = true: the activation tile is staged by the Tensor Memory Accelerator (one cp.async.bulk.tensor im2col load per
-// k-block lands 128 pixels x 32 channels, swizzled, zero-filled where the filter tap falls into the padding) and IS the A
-// tile; the producer warps only apply the BN/ReLU pre-op in place (PRE != 0) -- no global loads, no address / bounds
-// arithmetic.  K is enumerated per tap in 32-channel chunks (identical to the dense-quad order whenever the K channels are
-// a multiple of 32, which the host requires), stride 1, no up-sample.
-template <int PRE, int UP, bool VEC, bool TMA>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParams p, const __grid_constant__ CUtensorMap tmap) {
+template <int PRE, int UP, bool VEC>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-byte aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -240,12 +223,13 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
     float *s_scale = reinterpret_cast<float *>(sm + pre_off);
     float *s_shift = s_scale + p.KC * 32;
     const uint32_t bar_off = pre_off + (PRE >= 2 ? (uint32_t)p.KC * 32u * 8u : 0u);
-    // bars: [0..MS) full (the filling group's 128 producer arrivals [+ its expect_tx arrival for the weight bytes]),
-    // [MS..2MS) raw (TMA mode: the activation tile and the weights land there), [2MS..3MS) empty (one arrival per consumer
-    // warp)
+    // bars: [0..MS) full (the filling group's 128 producer arrivals + its expect_tx arrival for the weight bytes),
+    // [MS..2MS) spare, [2MS..3MS) empty (one arrival per consumer warp).  The spare set is initialised like the others:
+    // without those instructions ptxas places the consumers' k-block loops 208 bytes earlier, and that placement measured
+    // 2-7 % slower on the wide-tile dgrad layers (H100 SXM, 700 W), with identical loop bodies.
     const uint32_t bar0 = base + bar_off;
     auto full = [&](int s) { return bar0 + 8u * s; };
-    auto raw = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
+    auto spare = [&](int s) { return bar0 + 8u * (MAX_STAGES + s); };
     auto empty = [&](int s) { return bar0 + 8u * (2 * MAX_STAGES + s); };
     double *s_stat = reinterpret_cast<double *>(sm + bar_off + BAR_BYTES);    // [8 warps][2][n_tile], only when p.stat_sum
 
@@ -259,8 +243,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
-            mbar_init(full(s), TMA ? PRODUCER_THREADS : PRODUCER_THREADS + 1);
-            mbar_init(raw(s), 1);
+            mbar_init(full(s), PRODUCER_THREADS + 1);
+            mbar_init(spare(s), 1);
             mbar_init(empty(s), CONSUMER_THREADS / 32);
         }
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -277,8 +261,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
         // ===================== producers (two groups x 4 warps, alternating k-blocks) =====================
         setmaxnreg_dec<PRODUCER_REGS>();
         // The group that fills a k-block also stages its weight tile: right after the stage has been released, one lane
-        // issues the 1-D bulk async copy (cp.async.bulk) of the pre-packed, pre-split, pre-swizzled B hi/lo rows -- and,
-        // in TMA mode, the im2col load of the activation tile -- completing on an mbarrier.
+        // issues the 1-D bulk async copy (cp.async.bulk) of the pre-packed, pre-split, pre-swizzled B hi/lo rows,
+        // completing on an mbarrier.
         const int total_kb = my_tiles * KB;        // host guarantees < 2^31
         const int pt = threadIdx.x - CONSUMER_THREADS;
         const int grp = pt / PRODUCER_THREADS;     // producer group: global k-blocks gk == grp (mod 2)
@@ -297,102 +281,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
         const float *__restrict__ xg = p.x;
         // swizzled byte offset of (row r0 + 16 i, chunk) inside a tile = roff0 + i * 2048
         const uint32_t roff0 = (uint32_t)r0 * 128u + (uint32_t)((chunk ^ (r0 & 7)) << 4);
-        if constexpr (TMA) {
-            // ---- the raw tile lands in shared memory (TMA); apply the pre-op in place
-            const bool need_mask = AFF && taps > 1;        // zero padding is applied AFTER the BatchNorm/ReLU pre-op
-            int oyt[8], oxt[8];
-            int ti = 0, kb = grp, cur = -1;
-            int nt = 0, win0 = 0, tw = 0, th = 0, tn = 0;
-            while (kb >= KB) { kb -= KB; ++ti; }
-            int s_t = grp;
-            uint32_t ph_t = 0;
-            if (issuer) tma_prefetch_desc(&tmap);
-            const int mine_t = (total_kb - grp + 1) >> 1;
-            for (int it = 0; it < mine_t; ++it) {
-                if (ti != cur) {
-                    cur = ti;
-                    const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
-                    const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
-                    nt = tile - (int)m_tile * p.n_tiles;
-                    win0 = p.kwin ? nt * n_tile / p.kwin * p.kwin : 0;     // grouped: first channel of the K window
-                    // first output pixel of the tile -> base-pixel coordinate of the im2col walk
-                    const uint32_t m0 = m_tile * BLOCK_M;
-                    const uint32_t q = fdiv(m0, p.fd_wout);
-                    const uint32_t b = fdiv(q, p.fd_hout);
-                    tw = (int)(m0 - q * (uint32_t)p.Wout) - p.tma_adj;
-                    th = (int)(q - b * (uint32_t)p.Hout) - p.tma_adj;
-                    tn = (int)b;
-                    if (need_mask) {
-#pragma unroll
-                        for (int i = 0; i < 8; ++i) {
-                            const uint32_t m = m0 + (uint32_t)r0 + 16u * i;
-                            const uint32_t qi = fdiv(m, p.fd_wout);
-                            const uint32_t bi = fdiv(qi, p.fd_hout);
-                            oxt[i] = (int)(m - qi * (uint32_t)p.Wout) - p.pad;
-                            oyt[i] = (int)(qi - bi * (uint32_t)p.Hout) - p.pad;
-                        }
-                    }
-                }
-                int tap = 0, kc = kb;
-                if (taps > 1) { tap = (int)fdiv((uint32_t)kb, p.fd_kc); kc = kb - tap * p.KC; }
-                const int ky = (int)fdiv((uint32_t)tap, p.fd_kw), kx = tap - ky * KW;
-                const uint32_t stage = base + (uint32_t)s_t * stage_bytes;
-                // The raw barrier is re-armed only after the stage's previous use was consumed: a parity wait only tells
-                // adjacent phases apart.
-                mbar_wait(empty(s_t), ph_t ^ 1);
-                if (issuer) {
-                    mbar_arrive_expect_tx(raw(s_t), wbytes + (uint32_t)A_TILE_BYTES);
-                    tma_im2col_4d(stage, &tmap, win0 + kc * 32, tw, th, tn, raw(s_t), (uint16_t)(kx * dil),
-                                  (uint16_t)(ky * dil));
-                    bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + ((size_t)nt * KB + kb) * wbytes, wbytes, raw(s_t));
-                }
-                if constexpr (PRE != 0) {
-                    const int c = kc * 32 + chunk * 4;
-                    uint32_t live = 0xffu;
-                    if (need_mask) {
-                        live = 0;
-#pragma unroll
-                        for (int i = 0; i < 8; ++i)
-                            live |= (((unsigned)(oyt[i] + ky * dil) < (unsigned)Hin && (unsigned)(oxt[i] + kx * dil) < (unsigned)Win) ? 1u : 0u) << i;
-                    }
-                    float sc[4] = {1.f, 1.f, 1.f, 1.f}, sh[4] = {0.f, 0.f, 0.f, 0.f};
-                    if (AFF) {
-                        const float4 a4 = *reinterpret_cast<const float4 *>(s_scale + c);
-                        const float4 b4 = *reinterpret_cast<const float4 *>(s_shift + c);
-                        sc[0] = a4.x; sc[1] = a4.y; sc[2] = a4.z; sc[3] = a4.w;
-                        sh[0] = b4.x; sh[1] = b4.y; sh[2] = b4.z; sh[3] = b4.w;
-                    }
-                    const uint32_t a_st = stage + roff0;
-                    mbar_wait(raw(s_t), ph_t);
-#pragma unroll
-                    for (int i = 0; i < 8; ++i) {
-                        const float4 q4 = ld_shared_v4(a_st + (uint32_t)i * 2048u);
-                        float v[4] = {q4.x, q4.y, q4.z, q4.w};
-#pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            float a = v[e];
-                            if (AFF) {
-                                a = fmaf(a, sc[e], sh[e]);              // scale/shift are 0 beyond Cin
-                                if (RELU) a = fmaxf(a, 0.f);
-                                a = ((live >> i) & 1u) ? a : 0.f;
-                            } else if (RELU) {
-                                a = fmaxf(a, 0.f);
-                            }
-                            v[e] = a;
-                        }
-                        st_shared_v4(a_st + (uint32_t)i * 2048u, v[0], v[1], v[2], v[3]);
-                    }
-                    fence_proxy_async();
-                } else {
-                    mbar_wait(raw(s_t), ph_t);
-                }
-                mbar_arrive(full(s_t));
-                s_t += 2;
-                if (s_t >= S) { s_t -= S; ph_t ^= 1; }
-                kb += 2;
-                while (kb >= KB) { kb -= KB; ++ti; }
-            }
-        } else {
         // ---- cursor: (tile iteration, k-block in tile) of the next k-block this group fills; this lane's channel quad of
         //      that k-block is g = 8 kb + chunk -> (tap, quad in tap) by multiply-shift division
         // oyx[i]: the row's top-left source coordinate, (oy << 16) | (ox & 0xffff) -- one register per row instead of two
@@ -475,13 +363,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
         for (int it = 0; it < mine; ++it) {
             if (l_ti != cur_ti) set_tile(l_ti);
             const int w = cur_nt * KB + l_kb;      // the k-block's weight tile in wpack (host guarantees < 2^31)
-            uint32_t g = (uint32_t)(l_kb * 8 + chunk);
-            uint32_t tap = fdiv(g, p.fd_cq);
-            if (p.chunk_major) {                   // (chunk, tap) order: one tap per k-block, the chunk advances every `taps` k-blocks
-                const uint32_t kc = fdiv((uint32_t)l_kb, p.fd_taps);
-                tap = (uint32_t)l_kb - kc * (uint32_t)taps;
-                g = tap * (uint32_t)p.CQ + kc * 8u + (uint32_t)chunk;
-            }
+            const uint32_t g = (uint32_t)(l_kb * 8 + chunk);
+            const uint32_t tap = fdiv(g, p.fd_cq);
             const uint32_t ky = fdiv(tap, p.fd_kw);
             const int kx = (int)(tap - ky * (uint32_t)KW);
             const int dy = (int)ky * dil, dx = kx * dil;
@@ -542,7 +425,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
             cp_async_wait_dyn(0);
             publish_pending();
         }
-        }   // !TMA
     } else {
         // ===================== consumers: two warpgroups, rows [64 wg, 64 wg + 64) of every 128-pixel tile =========
         setmaxnreg_inc<CONSUMER_REGS>();
@@ -772,10 +654,8 @@ extern "C" long long bts_conv_packed_floats(int n_rows, int k_channels, int KH, 
 }
 
 extern "C" int bts_conv_pack_weights(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw,
-                                     int Cout, int Cin, int KH, int KW, int transpose_flip, int flags, float *wpack,
-                                     void *stream) {
+                                     int Cout, int Cin, int KH, int KW, int transpose_flip, float *wpack, void *stream) {
     if (!w || !wpack || Cout < 1 || Cin < 1 || KH < 1 || KW < 1) return BTS_EINVAL;
-    if ((flags & 1) && ((transpose_flip ? Cout : Cin) % 32)) return BTS_EINVAL;      // chunk-major needs whole 32-channel chunks
     if (!bts_aligned16(wpack)) return BTS_EALIGN;
     const int rows = transpose_flip ? Cin : Cout;
     const int n_tile = bts_conv_n_tile(rows);
@@ -785,7 +665,7 @@ extern "C" int bts_conv_pack_weights(const float *w, long long s_co, long long s
     const long long cap = (long long)bts_num_sms() * 16;
     if (grid > cap) grid = cap;
     pack_weights_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(w, s_co, s_ci, s_kh, s_kw, Cout, Cin, KH, KW,
-                                                                    transpose_flip, wpack, n_tile, n_tiles, 0, 1, flags);
+                                                                    transpose_flip, wpack, n_tile, n_tiles, 0, 1);
     BTS_LAUNCH_CHECK();
     return 0;
 }
@@ -824,8 +704,8 @@ extern "C" long long bts_conv_packed_floats_grouped(int width, int cpg, int KH, 
 }
 
 extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw,
-                                             int width, int cpg, int KH, int KW, int transpose_flip, int flags,
-                                             float *wpack, void *stream) {
+                                             int width, int cpg, int KH, int KW, int transpose_flip, float *wpack,
+                                             void *stream) {
     if (!w || !wpack || KH < 1 || KW < 1) return BTS_EINVAL;
     const int kwin = bts_conv_group_window(width, cpg);
     if (!kwin) return BTS_EINVAL;
@@ -836,59 +716,10 @@ extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, lon
     if (grid > cap) grid = cap;
     pack_weights_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(w, s_co, s_ci, s_kh, s_kw, width, width, KH, KW,
                                                                     transpose_flip, wpack, bts_conv_group_n_tile(kwin),
-                                                                    width / bts_conv_group_n_tile(kwin), kwin, cpg, flags);
+                                                                    width / bts_conv_group_n_tile(kwin), kwin, cpg);
     BTS_LAUNCH_CHECK();
     return 0;
 }
-
-// ---- TMA tensor map of the NHWC activation tensor, im2col mode (cuTensorMapEncodeIm2col through the runtime's driver
-//      entry-point query: no link-time dependency on libcuda)
-static int g_tma_mode = 0;      // 0 off, 1 on, 2 on with base-pixel coordinates NOT shifted by the lower corner, 3 on + strict
-
-typedef CUresult (*EncodeIm2colFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *,
-                                   const int *, const int *, cuuint32_t, cuuint32_t, const cuuint32_t *, CUtensorMapInterleave,
-                                   CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-static EncodeIm2colFn encode_im2col_fn() {
-    static EncodeIm2colFn fn = nullptr;
-    static bool tried = false;
-    if (!tried) {
-        tried = true;
-        void *ptr = nullptr;
-        cudaDriverEntryPointQueryResult qres;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeIm2col", &ptr, cudaEnableDefault, &qres) == cudaSuccess &&
-            qres == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<EncodeIm2colFn>(ptr);
-    }
-    return fn;
-}
-
-// x: NHWC fp32, pixel stride xs floats (a channel slice of a wider slab is fine), C channels visible to the loads
-static int make_im2col_map(CUtensorMap *map, const float *x, long long xs, int B, int H, int W, int C, int KH, int KW, int pad,
-                           int dil) {
-    EncodeIm2colFn fn = encode_im2col_fn();
-    if (!fn) return BTS_EINVAL;
-    const cuuint64_t gdim[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    const cuuint64_t gstr[3] = {(cuuint64_t)xs * 4, (cuuint64_t)xs * 4 * W, (cuuint64_t)xs * 4 * W * H};
-    const int lower[2] = {-pad, -pad};                                        // bounding box lower corner (W, H)
-    const int upper[2] = {pad - dil * (KW - 1), pad - dil * (KH - 1)};        // upper corner: last base pixel = last output pixel
-    const cuuint32_t estr[4] = {1, 1, 1, 1};
-    const CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float *>(x), gdim, gstr, lower, upper,
-                          /*channelsPerPixel=*/32, /*pixelsPerColumn=*/BLOCK_M, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                          CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? 0 : 700 + (int)r;
-}
-
-// 0: activation tiles loaded by the producer warps (LDG); 1: staged by TMA where eligible; 2: bring-up variant of 1
-extern "C" int bts_conv_set_tma(int mode) {
-    if (mode < 0 || mode > 3) return BTS_EINVAL;
-    g_tma_mode = mode;
-    return 0;
-}
-extern "C" int bts_conv_get_tma(void) { return g_tma_mode; }
-// the kernel has one producer layout, two groups of 4 warps: 0 (default) and 2 select it, anything else is refused
-extern "C" int bts_conv_set_producer_groups(int g) { return g == 0 || g == 2 ? 0 : BTS_EINVAL; }
-
 
 struct BnBwdArgs {
     const float *x; long long xs; const float *st; int relu;
@@ -899,7 +730,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
                          int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                          const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
                          long long out_pixel_stride, int act, int precision, double *stat_sum, double *stat_sumsq,
-                         void *stream, const BnBwdArgs *bnb = nullptr, int flags = 0) {
+                         void *stream, const BnBwdArgs *bnb = nullptr) {
     if (!x || !wpack || !out || B < 0 || Hs < 1 || Ws < 1 || Cin < 1 || Cout < 1 || KH < 1 || KW < 1 || stride < 1 ||
         pad < 0 || dil < 1)
         return BTS_EINVAL;
@@ -961,51 +792,28 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.stages = (SMEM_LIMIT - 1024 - BAR_BYTES - pre_bytes - stat_bytes) / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     if (p.stages < 2) return BTS_EINVAL;
-    p.chunk_major = (flags & 1) ? 1 : 0;
-    if (p.chunk_major && ((p.Cin % 32) || p.up)) return BTS_EINVAL;
-    if (p.chunk_major && p.stages > 3) p.stages = 3;   // leave most of the SM's 228 KB to L1: consecutive k-blocks of a chunk
-                                                        // re-read the same pixels' lines shifted by one tap
     const int smem = p.stages * p.stage_bytes + pre_bytes + BAR_BYTES + stat_bytes + 1024;
     const int sms = bts_num_sms();
     dim3 grid((unsigned)(p.total_tiles < sms ? p.total_tiles : sms));
     const bool vec = p.vec_ok;      // aligned base + pixel stride % 4 == 0 (a channel tail is masked in-kernel)
     cudaError_t err = cudaSuccess;
-    // ---- TMA-staged activation tiles (see the kernel's TMA template parameter): stride-1, non-up-sampled layers whose K
-    //      channels are a multiple of 32 (dense-quad K order == per-tap 32-channel chunks) and whose rows are 16-byte aligned
-    CUtensorMap tmap;
-    memset(&tmap, 0, sizeof(tmap));
-    bool use_tma = false;
-    p.tma_adj = 0;
-    p.fd_taps = make_fastdiv((uint32_t)(KH * KW));
-    p.fd_kc = make_fastdiv((uint32_t)p.KC);
-    if (g_tma_mode != 0 && !p.chunk_major && p.up == 0 && stride == 1 && p.vec_ok && (p.Cin % 32) == 0 && pad <= 127 &&
-        dil * (KH - 1) - pad <= 128 && dil * (KW - 1) - pad <= 128 && dil * (KH - 1) <= 255 && dil * (KW - 1) <= 255) {
-        const int rc = make_im2col_map(&tmap, x, x_pixel_stride, B, Hs, Ws, kwin ? Cin : p.Cin, KH, KW, pad, dil);
-        if (rc == 0) {
-            use_tma = true;
-            p.tma_adj = g_tma_mode == 2 ? 0 : pad;      // mode 2: alternative coordinate convention (bring-up switch)
-        } else if (g_tma_mode == 3) {
-            return rc;                                   // forced: report why the map could not be built
-        }
-    }
-#define BTS_LAUNCH(PRE, UP, VEC, TMA)                                                                              \
+#define BTS_LAUNCH(PRE, UP, VEC)                                                                                   \
     do {                                                                                                           \
         static bool attr_set_[BTS_MAX_DEVICES] = {};                                                               \
         bool &attr_set = attr_set_[bts_cur_device()];                                                              \
         if (!attr_set) {                                                                                           \
-            err = cudaFuncSetAttribute(conv_tc_kernel<PRE, UP, VEC, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize,    \
+            err = cudaFuncSetAttribute(conv_tc_kernel<PRE, UP, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
                                        SMEM_LIMIT);                                                                \
             if (err != cudaSuccess) return (int)err;                                                               \
             attr_set = true;                                                                                       \
         }                                                                                                          \
-        conv_tc_kernel<PRE, UP, VEC, TMA><<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(p, tmap);                    \
+        conv_tc_kernel<PRE, UP, VEC><<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(p);                        \
     } while (0)
-#define BTS_DISPATCH_UV(PRE)                                  \
-    do {                                                      \
-        if (use_tma) BTS_LAUNCH(PRE, 0, true, true);                                                            \
-        else if (p.up == 2) { if (vec) BTS_LAUNCH(PRE, 2, true, false); else BTS_LAUNCH(PRE, 2, false, false); }    \
-        else if (p.up) { if (vec) BTS_LAUNCH(PRE, 1, true, false); else BTS_LAUNCH(PRE, 1, false, false); }    \
-        else { if (vec) BTS_LAUNCH(PRE, 0, true, false); else BTS_LAUNCH(PRE, 0, false, false); }              \
+#define BTS_DISPATCH_UV(PRE)                                                                                       \
+    do {                                                                                                           \
+        if (p.up == 2) { if (vec) BTS_LAUNCH(PRE, 2, true); else BTS_LAUNCH(PRE, 2, false); }                      \
+        else if (p.up) { if (vec) BTS_LAUNCH(PRE, 1, true); else BTS_LAUNCH(PRE, 1, false); }                      \
+        else { if (vec) BTS_LAUNCH(PRE, 0, true); else BTS_LAUNCH(PRE, 0, false); }                                \
     } while (0)
     switch (pre) {
         case 0: BTS_DISPATCH_UV(0); break;
@@ -1049,10 +857,10 @@ extern "C" int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, 
                                int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
                                const float *wpack, int Cout, const float *pre_scale, const float *pre_shift, int pre_relu,
                                float *out, long long out_pixel_stride, int act, int precision, double *stat_sum,
-                               double *stat_sumsq, int flags, void *stream) {
+                               double *stat_sumsq, void *stream) {
     return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
                          Cout, pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq,
-                         stream, nullptr, flags);
+                         stream);
 }
 
 // descs: device array of n PackDesc (layout above; built by the host side once per model), total = sum of packed_floats / 2
@@ -1075,8 +883,8 @@ extern "C" int bts_conv_fwd_bnbwd(const float *x, long long x_pixel_stride, int 
                                   int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
                                   const float *wpack, int Cout, float *out, long long out_pixel_stride, int precision,
                                   const float *x_bn, long long x_bn_stride, const float *bn_st, int relu, double *S1,
-                                  double *S2, int flags, void *stream) {
+                                  double *S2, void *stream) {
     BnBwdArgs a{x_bn, x_bn_stride, bn_st, relu};
     return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
-                         Cout, nullptr, nullptr, 0, out, out_pixel_stride, 0, precision, S1, S2, stream, &a, flags);
+                         Cout, nullptr, nullptr, 0, out, out_pixel_stride, 0, precision, S1, S2, stream, &a);
 }

@@ -54,17 +54,6 @@ __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void *src, uin
                  "l"(src), "r"(bytes), "r"(bar)
                  : "memory");
 }
-// TMA im2col load (cp.async.bulk.tensor ... .im2col): `pixelsPerColumn` consecutive base pixels starting at
-// tensor coordinate (w, h, n), each shifted by the filter offset (off_w, off_h), `channelsPerPixel` channels from c; pixels
-// that fall outside the tensor (the convolution's zero padding) arrive as zeros.  Completes `bytes` on the mbarrier.
-__device__ __forceinline__ void tma_im2col_4d(uint32_t dst, const void *tmap, int c, int w, int h, int n, uint32_t bar,
-                                              uint16_t off_w, uint16_t off_h) {
-    asm volatile(
-        "cp.async.bulk.tensor.4d.shared::cluster.global.im2col.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6], "
-        "{%7, %8};" ::"r"(dst),
-        "l"(tmap), "r"(c), "r"(w), "r"(h), "r"(n), "r"(bar), "h"(off_w), "h"(off_h)
-        : "memory");
-}
 // plain (tiled) 2-D tensor load: coordinates {c0 = innermost, c1}; out-of-range elements are zero-filled
 __device__ __forceinline__ void tma_tile_2d(uint32_t dst, const void *tmap, int c0, int c1, uint32_t bar) {
     asm volatile(

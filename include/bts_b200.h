@@ -102,12 +102,8 @@ int bts_plane_head_bwd(const float *d_scaled, const float *d_ds, const float *c3
  *   bts_conv_n_tile(Cout) -> the N tile the engine uses for that many output channels. */
 int bts_conv_n_tile(int Cout);
 long long bts_conv_packed_floats(int n_rows, int k_channels, int KH, int KW);
-/* flags bit 0 = chunk-major K order (K channels % 32 == 0): k-block = (32-channel chunk, tap) with the taps innermost, so
- * that consecutive k-blocks re-read the same pixels' cache lines (hits in L1 instead of nine L2 reads per element); pass the
- * same flags to bts_conv_fwd_ex / bts_conv_fwd_bnbwd. */
 int bts_conv_pack_weights(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw,
-                          int Cout, int Cin, int KH, int KW, int transpose_flip, int flags, float *wpack,
-                          void *stream);
+                          int Cout, int Cin, int KH, int KW, int transpose_flip, float *wpack, void *stream);
 int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
                  int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                  const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
@@ -133,17 +129,7 @@ int bts_conv_fwd_stats(const float *x, long long x_pixel_stride, int B, int Hs, 
 int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
                     int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                     const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
-                    int act, int precision, double *stat_sum, double *stat_sumsq, int flags, void *stream);
-/* Staging of the activation tiles of bts_conv_fwd*: 0 = the producer warps load them (LDG + pre-op in registers),
- * 1 = TMA im2col loads (cp.async.bulk.tensor im2col; zero padding by out-of-bounds fill) land the raw tile in
- * shared memory as the A operand and the producers only apply the pre-op in place -- used for stride-1, non-up-sampled layers
- * whose K channels are a multiple of 32 and whose rows are 16-byte aligned, every other layer keeps mode 0 automatically.
- * (2, 3: bring-up variants.)  Process-wide setting. */
-int bts_conv_set_tma(int mode);
-int bts_conv_get_tma(void);
-/* activation-producer groups of the conv engine (4 warps each): the engine runs two groups; 0 (default) and 2 are
- * accepted, any other value returns BTS_EINVAL. */
-int bts_conv_set_producer_groups(int groups);
+                    int act, int precision, double *stat_sum, double *stat_sumsq, void *stream);
 /* Tuning / bring-up switches of the narrow-output wgrad (csrc/wgrad2_tc.cu).  set_tma(0): the producers load the operands
  * from global memory (round-1 path) instead of the TMA landing ring; set_min_pixels(n): smallest map (input pixels) routed to
  * this kernel (default 12000, n < 0 restores it; tests pass 0 to reach it with small shapes). */
@@ -159,7 +145,7 @@ int bts_wgrad2_set_pointwise(int on);        /* 1 (default): 1x1 layers with 64 
 int bts_conv_fwd_bnbwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
                        int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                        float *out, long long out_pixel_stride, int precision, const float *x_bn, long long x_bn_stride,
-                       const float *bn_st, int relu, double *S1, double *S2, int flags, void *stream);
+                       const float *bn_st, int relu, double *S1, double *S2, void *stream);
 int bts_bn_bwd_coef(const double *S1, const double *S2, long long M, int C, const float *scale, const float *mean,
                     const float *invstd, float *coef, void *stream);
 /* grouped 3x3 (ResNeXt: 32 groups of cpg channels): w is (width, cpg, KH, KW).  bts_conv_group_window -> the diagonal block
@@ -169,7 +155,7 @@ int bts_conv_group_window(int width, int cpg);
 int bts_conv_group_n_tile(int kwin);
 long long bts_conv_packed_floats_grouped(int width, int cpg, int KH, int KW);
 int bts_conv_pack_weights_grouped(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw, int width,
-                                  int cpg, int KH, int KW, int transpose_flip, int flags, float *wpack, void *stream);
+                                  int cpg, int KH, int KW, int transpose_flip, float *wpack, void *stream);
 int bts_conv_wgrad_grouped_plan(int B, int Hout, int Wout, int width, int cpg, int KH, int KW, int *splitK_out,
                                 long long *workspace_floats);
 int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int width, int cpg, int KH, int KW,

@@ -46,6 +46,6 @@ def _conv_kernel_resources():
 
 def test_conv_kernel_fits_registers_without_spills():
     res = _conv_kernel_resources()
-    assert res, "no conv_tc_kernel in the library"
+    assert len(res) == 24, "expected 24 conv_tc_kernel instantiations, found %d" % len(res)
     bad = {k: v for k, v in res.items() if v[0] > 128 or v[1] != 0}
     assert not bad, "conv_tc_kernel instantiations over 128 registers or with a stack frame (REG, STACK): %s" % bad

@@ -1,8 +1,8 @@
 """GPU parity of the conv engine's wide output tiles (n-tiles of 80..128 channels, bts_conv_n_tile) against torch fp64 on
 the CPU, at the 2e-5 output-scale bar of tests/test_conv_gpu.py: forward and dgrad widths, the BatchNorm/ReLU pre-op with
 padding, the folded x2 up-sample, the zero-stuffed source of a stride-2 dgrad, channel tails, channel slices of wider slabs,
-the epilogue statistics and the BatchNorm-backward epilogue, fast mode, TMA staging, a grouped operator with a 128-wide
-window, and a launch with fewer tiles than SMs."""
+the epilogue statistics and the BatchNorm-backward epilogue, fast mode, a grouped operator with a 128-wide window, and a
+launch with fewer tiles than SMs."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -157,37 +157,6 @@ def test_wide_fast_mode_is_labelled_and_less_exact(Cout):
     e3 = _err(conv.conv2d_tc(xc, w.cuda(), 1, 1, 1), ref)
     e1 = _err(conv.conv2d_tc(xc, w.cuda(), 1, 1, 1, precision=1), ref)
     assert e3 < 2e-5 and 1e-5 < e1 < 5e-3
-
-
-@pytest.fixture
-def tma():
-    from bts_b200 import _lib, conv
-    L = _lib.lib()
-    prev, prev_cm = L.bts_conv_get_tma(), conv.CHUNK_MAJOR
-    conv.CHUNK_MAJOR = False
-    yield L
-    L.bts_conv_set_tma(prev)
-    conv.CHUNK_MAJOR = prev_cm
-
-
-@pytest.mark.parametrize("Cout,pre", [(96, True), (128, False), (192, True), (448, False)])
-def test_wide_tma_staged(tma, Cout, pre):
-    from bts_b200 import conv
-    g = torch.Generator().manual_seed(Cout + pre)
-    Cin = 96
-    x = torch.randn(2, Cin, 9, 11, generator=g)
-    w = torch.randn(Cout, Cin, 3, 3, generator=g) / (Cin * 9) ** 0.5
-    xd = x.double()
-    kw = {}
-    if pre:
-        sc, sh = _bn(Cin, g)
-        xd = F.relu(xd * sc.double().view(1, -1, 1, 1) + sh.double().view(1, -1, 1, 1))
-        kw = dict(pre_scale=sc.cuda(), pre_shift=sh.cuda(), pre_relu=True)
-    ref = F.conv2d(xd, w.double(), None, 1, 1, 1)
-    tma.bts_conv_set_tma(3)                    # strict: a tensor-map failure is an error
-    y = conv.conv2d_tc(_cl(x), w.cuda(), 1, 1, 1, **kw)
-    torch.cuda.synchronize()
-    assert _err(y, ref) < 4e-5                 # the bar of tests/test_zz_conv_tma_gpu.py
 
 
 def test_grouped_operator_with_a_128_wide_window():

@@ -97,11 +97,3 @@ def test_packed_operator_sizes_and_group_windows():
         assert L.bts_conv_group_window(width, cpg) == 128
     assert L.bts_conv_group_window(96, 3) == 96                   # narrower widths: one window
     assert L.bts_conv_group_window(100, 3) == 0                   # width not a multiple of the group size: refused
-
-
-def test_switches_validate_their_arguments():
-    L = _lib()
-    assert L.bts_conv_set_producer_groups(3) != 0
-    assert L.bts_conv_set_producer_groups(0) == 0
-    assert L.bts_conv_set_tma(7) != 0
-    assert L.bts_conv_set_tma(0) == 0
