@@ -133,8 +133,15 @@ SIGNATURES = {
     "bts_conv_pw_fwd_eligible": [_i, _i],
     "bts_conv_pw_fwd": [_p, _ll, _ll, _i, _p, _ll, _ll, _i, _i, _p, _ll, _p],
     "bts_conv_pw_wgrad": [_p, _ll, _p, _ll, _ll, _i, _i, _p, _p, _ll, _ll, _p],
+    "bts_bn_add": [_p, _ll, _ll, _i, _p, _p, _p, _ll, _p, _ll, _p],
+    "bts_dw3x3_fwd_workspace_floats": [_i, _i, _i, _i, _i],
+    "bts_dw3x3_fwd": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _ll, _ll, _p, _p, _p, _p, _p, _ll, _p, _p, _p, _p],
+    "bts_dw3x3_dgrad": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _ll, _ll, _p, _ll, _p],
+    "bts_dw3x3_wgrad_workspace_floats": [_i, _i, _i, _i, _i],
+    "bts_dw3x3_wgrad": [_p, _ll, _p, _ll, _i, _i, _i, _i, _i, _p, _p, _p, _p, _ll, _ll, _ll, _p],
 }
-RESTYPES = {"bts_conv_packed_floats": ctypes.c_longlong, "bts_conv_packed_floats_grouped": ctypes.c_longlong, "bts_conv_pw_wgrad_workspace_floats": ctypes.c_longlong}
+RESTYPES = {"bts_conv_packed_floats": ctypes.c_longlong, "bts_conv_packed_floats_grouped": ctypes.c_longlong, "bts_conv_pw_wgrad_workspace_floats": ctypes.c_longlong,
+            "bts_dw3x3_fwd_workspace_floats": ctypes.c_longlong, "bts_dw3x3_wgrad_workspace_floats": ctypes.c_longlong}
 
 
 def lib():

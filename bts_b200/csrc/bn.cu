@@ -15,17 +15,22 @@
 
 namespace {
 
+// the backward mask of the activation after y = x*scale + shift: 0 none, 1 ReLU [y > 0], 2 ReLU6 [0 < y < 6] (strict on
+// both sides, as torch's hardtanh_backward)
+__device__ __forceinline__ bool act_pass(int act, float y) { return act == 0 || (y > 0.f && (act == 1 || y < 6.f)); }
+
 // Column reductions over NHWC: a 256-thread block covers up to 256 channels (64 channel quads) x `rows` pixels; with
 // fewer channels the spare threads take extra pixel rows.  Four independent 16-byte loads per tensor are in flight per
 // thread; the row groups of a block are combined in shared memory, then ONE fp64 atomic per channel per block.
 // MODE 0: forward statistics; 1: backward sums; 2: backward sums AND out += [y>0]*scale*g in the same pass (the part of dx
 // that does not depend on the sums -- the k1*x + k0 remainder is deferred, see bts_bn_relu_bwd_fused).
+// `act` is the activation code after the normalisation: 0 none, 1 ReLU, 2 ReLU6 (see act_pass).
 template <int MODE>
 __global__ void __launch_bounds__(256) bn_reduce_kernel(const float *__restrict__ x, long long xs, const float *__restrict__ g,
                                                         long long gs, long long M, int C, int rows,
                                                         const float *__restrict__ scale, const float *__restrict__ shift,
                                                         const float *__restrict__ mean, const float *__restrict__ invstd,
-                                                        double *__restrict__ acc0, double *__restrict__ acc1, int relu,
+                                                        double *__restrict__ acc0, double *__restrict__ acc1, int act,
                                                         float *out, long long os) {
     constexpr bool BWD = MODE != 0;
     constexpr bool ACC = MODE == 2;
@@ -60,7 +65,7 @@ __global__ void __launch_bounds__(256) bn_reduce_kernel(const float *__restrict_
                     a1[e] = fmaf(xv[e], xv[e], a1[e]);
                 } else {
                     const float y = fmaf(xv[e], sc[e], sh[e]);
-                    const float gm = (!relu || y > 0.f) ? gv[e] : 0.f;
+                    const float gm = act_pass(act, y) ? gv[e] : 0.f;
                     a0[e] += gm;
                     a1[e] = fmaf(gm, (xv[e] - mu[e]) * is[e], a1[e]);
                     if (ACC) ov[e] = fmaf(sc[e], gm, ov[e]);
@@ -237,13 +242,14 @@ __global__ void bn_fold_kernel(int C, const float *__restrict__ gamma, const flo
     invstd[c] = is;
 }
 
-// dx = [y>0]*scale*g + k1*x + k0  (train; coef = (k0,k1) from bn_bwd_coef_kernel)   or   [y>0]*scale*g  (coef == null)
+// dx = [y>0]*scale*g + k1*x + k0  (train; coef = (k0,k1) from bn_bwd_coef_kernel)   or   [y>0]*scale*g  (coef == null);
+// [y>0] stands for the mask of activation code `act` (act_pass)
 __global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const float *__restrict__ x, long long xs,
                                                                 const float *__restrict__ g, long long gs, long long M,
                                                                 int C, const float *__restrict__ scale,
                                                                 const float *__restrict__ shift, const float *__restrict__ coef,
                                                                 float *__restrict__ out, long long os, int accumulate,
-                                                                int relu) {
+                                                                int act) {
     const int cq = (C + 3) >> 2;
     const long long total = M * cq;
     const bool vec = ((xs & 3) == 0) && ((gs & 3) == 0) && ((os & 3) == 0) && ((((uintptr_t)x) & 15) == 0) &&
@@ -288,7 +294,7 @@ __global__ void __launch_bounds__(256) bn_relu_bwd_apply_kernel(const float *__r
 #pragma unroll
         for (int e = 0; e < 4; ++e) {
             const float y = fmaf(xv[e], sc[e], sh[e]);
-            float d = (!relu || y > 0.f) ? sc[e] * gv[e] : 0.f;
+            float d = act_pass(act, y) ? sc[e] * gv[e] : 0.f;
             d += fmaf(xv[e], k1[e], k0[e]);
             r[e] = ov[e] + d;
         }
@@ -369,7 +375,7 @@ extern "C" int bts_bn_fold(int C, const float *gamma, const float *beta, float e
 
 extern "C" int bts_bn_bwd_reduce(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
                                  long long M, int C, const float *scale, const float *shift, const float *mean,
-                                 const float *invstd, int relu, double *S1, double *S2, float *coef, void *stream) {
+                                 const float *invstd, int act, double *S1, double *S2, float *coef, void *stream) {
     if (!x || !g || !scale || !shift || !mean || !invstd || !S1 || !S2 || !coef || M < 1 || C < 1) return BTS_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t e;
@@ -383,7 +389,7 @@ extern "C" int bts_bn_bwd_reduce(const float *x, long long x_pixel_stride, const
     const int rows = reduce_rows(M, cg);
     dim3 grid((unsigned)((M + rows - 1) / rows), (unsigned)cg);
     bn_reduce_kernel<1><<<grid, 256, 0, st>>>(x, x_pixel_stride, g, g_pixel_stride, M, C, rows, scale, shift, mean, invstd,
-                                              S1, S2, relu, nullptr, 0);
+                                              S1, S2, act, nullptr, 0);
     BTS_LAUNCH_CHECK();
     bn_bwd_coef_kernel<<<(C + 127) / 128, 128, 0, st>>>(S1, S2, M, C, scale, mean, invstd, coef);
     BTS_LAUNCH_CHECK();
@@ -451,7 +457,7 @@ extern "C" int bts_bn_relu_bwd_reduce(const float *x, long long x_pixel_stride, 
 }
 
 extern "C" int bts_bn_bwd_apply(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
-                                long long M, int C, const float *scale, const float *shift, const float *coef, int relu,
+                                long long M, int C, const float *scale, const float *shift, const float *coef, int act,
                                 float *out, long long out_pixel_stride, int accumulate, void *stream) {
     if (!x || !g || !scale || !shift || !out || M < 1 || C < 1) return BTS_EINVAL;
     const long long total = M * ((C + 3) / 4);
@@ -460,7 +466,7 @@ extern "C" int bts_bn_bwd_apply(const float *x, long long x_pixel_stride, const 
     if (grid > cap) grid = cap;
     bn_relu_bwd_apply_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(x, x_pixel_stride, g, g_pixel_stride, M, C, scale,
                                                                           shift, coef, out, out_pixel_stride, accumulate,
-                                                                          relu);
+                                                                          act);
     BTS_LAUNCH_CHECK();
     return 0;
 }

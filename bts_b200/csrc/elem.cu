@@ -3,7 +3,8 @@
 // sm_90a, HBM-bound.  All tensors are fp32 NHWC with an explicit pixel stride, so a channel slice of a wider slab is
 // read or written in place (concat = one vectorised slice copy per input instead of CatArrayBatchedCopy).
 //
-//   bts_bn_apply       out = x*scale + shift [ReLU]                    BatchNorm apply (train or folded eval stats)
+//   bts_bn_apply       out = act(x*scale + shift)                      BatchNorm apply (train or folded eval stats),
+//                      act 0 none, 1 ReLU, 2 ReLU6
 //   bts_elu_bwd        out = gy * (y > 0 ? 1 : y + 1)                  ELU'(a) expressed through the saved OUTPUT y
 //   bts_upsample2_sum  out[b,y,x,c] = sum of the 2x2 block of g        backward of the nearest x2 up-sample folded into
 //                      [* (x > 0) when relu_src != null]               upconv's im2col map (+ the ReLU in front of upconv5)
@@ -31,7 +32,7 @@ __device__ __forceinline__ bool al16(const void *p) { return (((uintptr_t)p) & 1
 
 __global__ void __launch_bounds__(TPB) bn_apply_kernel(const float *__restrict__ x, long long xs, long long M, int C,
                                                        const float *__restrict__ scale, const float *__restrict__ shift,
-                                                       int relu, float *__restrict__ out, long long os) {
+                                                       int act, float *__restrict__ out, long long os) {
     const int cq = (C + 3) >> 2;
     const long long total = M * cq;
     const bool vec = ((C & 3) == 0) && ((xs & 3) == 0) && ((os & 3) == 0) && al16(x) && al16(out) && al16(scale) && al16(shift);
@@ -43,12 +44,14 @@ __global__ void __launch_bounds__(TPB) bn_apply_kernel(const float *__restrict__
             const float4 s = __ldg(reinterpret_cast<const float4 *>(scale + c));
             const float4 h = __ldg(reinterpret_cast<const float4 *>(shift + c));
             float4 r = make_float4(fmaf(q.x, s.x, h.x), fmaf(q.y, s.y, h.y), fmaf(q.z, s.z, h.z), fmaf(q.w, s.w, h.w));
-            if (relu) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f); }
+            if (act) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f); }
+            if (act == 2) { r.x = fminf(r.x, 6.f); r.y = fminf(r.y, 6.f); r.z = fminf(r.z, 6.f); r.w = fminf(r.w, 6.f); }
             *reinterpret_cast<float4 *>(out + m * os + c) = r;
         } else {
             for (int e = 0; e < 4 && c + e < C; ++e) {
                 float r = fmaf(x[m * xs + c + e], scale[c + e], shift[c + e]);
-                if (relu) r = fmaxf(r, 0.f);
+                if (act) r = fmaxf(r, 0.f);
+                if (act == 2) r = fminf(r, 6.f);
                 out[m * os + c + e] = r;
             }
         }
@@ -200,7 +203,9 @@ __global__ void __launch_bounds__(TPB) avgpool2_kernel(const float *__restrict__
 }
 
 // ResNet / ResNeXt bottleneck tail (torchvision Bottleneck.forward: out = relu(bn3(conv3) + identity)):
-//   out = max(x*scale + shift + res, 0)
+//   out = max(x*scale + shift + res, 0);  RELU = false: out = x*scale + shift + res, the MobileNetV2 inverted-residual
+//   tail x + bn3(conv3(.)) (torchvision InvertedResidual with use_res_connect)
+template <bool RELU>
 __global__ void __launch_bounds__(TPB) bn_add_relu_kernel(const float *__restrict__ x, long long xs, long long M, int C,
                                                           const float *__restrict__ scale, const float *__restrict__ shift,
                                                           const float *__restrict__ res, long long rs,
@@ -219,11 +224,13 @@ __global__ void __launch_bounds__(TPB) bn_add_relu_kernel(const float *__restric
             const float4 h = __ldg(reinterpret_cast<const float4 *>(shift + c));
             float4 r = make_float4(fmaf(q.x, s.x, h.x) + r0.x, fmaf(q.y, s.y, h.y) + r0.y, fmaf(q.z, s.z, h.z) + r0.z,
                                    fmaf(q.w, s.w, h.w) + r0.w);
-            r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f);
+            if (RELU) { r.x = fmaxf(r.x, 0.f); r.y = fmaxf(r.y, 0.f); r.z = fmaxf(r.z, 0.f); r.w = fmaxf(r.w, 0.f); }
             *reinterpret_cast<float4 *>(out + m * os + c) = r;
         } else {
-            for (int e = 0; e < 4 && c + e < C; ++e)
-                out[m * os + c + e] = fmaxf(fmaf(x[m * xs + c + e], scale[c + e], shift[c + e]) + res[m * rs + c + e], 0.f);
+            for (int e = 0; e < 4 && c + e < C; ++e) {
+                const float r = fmaf(x[m * xs + c + e], scale[c + e], shift[c + e]) + res[m * rs + c + e];
+                out[m * os + c + e] = RELU ? fmaxf(r, 0.f) : r;
+            }
         }
     }
 }
@@ -312,10 +319,10 @@ __global__ void __launch_bounds__(TPB) maxpool3s2_bwd_kernel(const float *__rest
 }  // namespace
 
 extern "C" int bts_bn_apply(const float *x, long long x_pixel_stride, long long M, int C, const float *scale,
-                            const float *shift, int relu, float *out, long long out_pixel_stride, void *stream) {
+                            const float *shift, int act, float *out, long long out_pixel_stride, void *stream) {
     if (!x || !scale || !shift || !out || M < 1 || C < 1) return BTS_EINVAL;
     bn_apply_kernel<<<stream_grid(M * ((C + 3) / 4)), TPB, 0, (cudaStream_t)stream>>>(x, x_pixel_stride, M, C, scale, shift,
-                                                                                       relu, out, out_pixel_stride);
+                                                                                       act, out, out_pixel_stride);
     BTS_LAUNCH_CHECK();
     return 0;
 }
@@ -376,8 +383,19 @@ extern "C" int bts_bn_add_relu(const float *x, long long x_pixel_stride, long lo
                                const float *shift, const float *res, long long res_pixel_stride, float *out,
                                long long out_pixel_stride, void *stream) {
     if (!x || !scale || !shift || !res || !out || M < 1 || C < 1) return BTS_EINVAL;
-    bn_add_relu_kernel<<<stream_grid(M * ((C + 3) / 4)), TPB, 0, (cudaStream_t)stream>>>(x, x_pixel_stride, M, C, scale, shift, res,
-                                                                                          res_pixel_stride, out, out_pixel_stride);
+    bn_add_relu_kernel<true><<<stream_grid(M * ((C + 3) / 4)), TPB, 0, (cudaStream_t)stream>>>(x, x_pixel_stride, M, C, scale,
+                                                                                                shift, res, res_pixel_stride, out,
+                                                                                                out_pixel_stride);
+    BTS_LAUNCH_CHECK();
+    return 0;
+}
+
+extern "C" int bts_bn_add(const float *x, long long x_pixel_stride, long long M, int C, const float *scale, const float *shift,
+                          const float *res, long long res_pixel_stride, float *out, long long out_pixel_stride, void *stream) {
+    if (!x || !scale || !shift || !res || !out || M < 1 || C < 1) return BTS_EINVAL;
+    bn_add_relu_kernel<false><<<stream_grid(M * ((C + 3) / 4)), TPB, 0, (cudaStream_t)stream>>>(x, x_pixel_stride, M, C, scale,
+                                                                                                 shift, res, res_pixel_stride,
+                                                                                                 out, out_pixel_stride);
     BTS_LAUNCH_CHECK();
     return 0;
 }

@@ -5,10 +5,14 @@ conv engine (ELU in the epilogue, ReLU / BN-apply + ReLU in the A-operand prolog
 run as one of the streaming NHWC kernels of csrc/elem.cu / csrc/bn.cu:
 
   conv_act       y = act(conv(pre_relu?(up2?(x))))        upconv (bts.py:69-80), iconvs (:156-192), reduction chains (:83-108)
-  bn_act         y = BN(x) [ReLU]                          decoder BNs (:154-182), torchvision norm0(+relu0) / norm5
+  bn_act         y = BN(x) [ReLU | ReLU6]                  decoder BNs (:154-182), torchvision norm0(+relu0) / norm5,
+                                                           mobilenet_v2's stem and last Conv2dNormActivation
   bn_relu_conv   y = conv(ReLU(BN(x)))                     atrous_conv halves (:51-66), DenseNet transitions
   cat_nhwc       channel concat into a 16-byte-aligned slab (the nine torch.cat of bts.forward); backward = views
   avgpool2       2x2 average pool of the transitions
+  inverted_residual  one torchvision InvertedResidual (mobilenet_v2, bts.py:297-300) as a single Function: 1x1 expand
+                 with BN1 statistics from the engine epilogue, depthwise 3x3 with BN1 + ReLU6 in its prologue and BN2
+                 statistics in its epilogue (csrc/dwconv.cu), BN2 + ReLU6, 1x1 project, BN3 [+ residual]
 
 Each unit is a torch.autograd.Function whose backward launches our kernels too (ELU', BN reductions, wgrad / dgrad on
 the engine, 2x2 gradient fold of the up-sample).  Parameters stay the nn.Modules' own, BatchNorm running statistics are
@@ -71,8 +75,9 @@ def bn_uses_batch_stats(bn):
     return bn.training or bn.running_mean is None
 
 
-def bn_backward(x, g, st, use_stats, relu, out=None, accumulate=False):
-    """d/dx of [relu](bn(x)) given g = d/d(output); returns (dx, S) with S = (dbeta, dgamma) as fp64 [2,C]"""
+def bn_backward(x, g, st, use_stats, act, out=None, accumulate=False):
+    """d/dx of act(bn(x)) given g = d/d(output), activation code `act`: 0 none, 1 ReLU, 2 ReLU6 (a bool is 0 / 1);
+    returns (dx, S) with S = (dbeta, dgamma) as fp64 [2,C]"""
     x, xs = _nhwc(x)
     g, gs = _nhwc(g)
     B, C, H, W = x.shape
@@ -86,9 +91,9 @@ def bn_backward(x, g, st, use_stats, relu, out=None, accumulate=False):
     S = torch.empty((2, C), device=x.device, dtype=torch.float64)
     coef = torch.empty((2, C), device=x.device, dtype=torch.float32)
     _lib.check(L.bts_bn_bwd_reduce(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]), _ptr(st[2]), _ptr(st[3]),
-                                   int(relu), _ptr(S[0]), _ptr(S[1]), _ptr(coef), _stream()), "bts_bn_bwd_reduce")
+                                   int(act), _ptr(S[0]), _ptr(S[1]), _ptr(coef), _stream()), "bts_bn_bwd_reduce")
     _lib.check(L.bts_bn_bwd_apply(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]),
-                                  _ptr(coef) if use_stats else None, int(relu), _ptr(out), os_, int(accumulate), _stream()),
+                                  _ptr(coef) if use_stats else None, int(act), _ptr(out), os_, int(accumulate), _stream()),
                "bts_bn_bwd_apply")
     _lib.count(3)
     return out, S
@@ -163,33 +168,39 @@ def conv_act(x, weight, padding=0, dilation=1, pre_relu=False, up=False, act=Non
 # ------------------------------------------------------------------------------------------------ BatchNorm (+ ReLU)
 class _BnAct(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, x, gamma, beta, bn, relu):
+    def forward(ctx, x, gamma, beta, bn, act):
         x, xs = _nhwc(x)
         B, C, H, W = x.shape
         n = B * H * W
         batch = bn_uses_batch_stats(bn)
         st = bn_finalize(bn_stats(x) if batch else None, n, bn, gamma, beta, batch)
         y = _new(B, C, H, W, x.device)
-        _lib.check(_lib.lib().bts_bn_apply(_ptr(x), xs, n, C, _ptr(st[0]), _ptr(st[1]), int(relu), _ptr(y), C, _stream()),
+        _lib.check(_lib.lib().bts_bn_apply(_ptr(x), xs, n, C, _ptr(st[0]), _ptr(st[1]), act, _ptr(y), C, _stream()),
                    "bts_bn_apply")
         _lib.count()
-        ctx.cfg = (batch, relu)
+        ctx.cfg = (batch, act)
         ctx.save_for_backward(x, st)
         return y
 
     @staticmethod
     def backward(ctx, gy):
         x, st = ctx.saved_tensors
-        batch, relu = ctx.cfg
-        gx, S = bn_backward(x, gy, st, batch, relu)
+        batch, act = ctx.cfg
+        gx, S = bn_backward(x, gy, st, batch, act)
         return (gx if ctx.needs_input_grad[0] else None, S[1].float() if ctx.needs_input_grad[1] else None,
                 S[0].float() if ctx.needs_input_grad[2] else None, None, None)
 
 
-def bn_act(x, bn, relu=False):
+ACT_CODES = {None: 0, "relu": 1, "relu6": 2}
+
+
+def bn_act(x, bn, relu=False, act=None):
     """nn.BatchNorm2d `bn` applied to x (batch statistics + running-stat update in train mode, folded running
-    statistics in eval mode), optionally followed by ReLU -- 3 streaming kernels forward, 3 backward"""
-    return _BnAct.apply(x, bn.weight, bn.bias, bn, bool(relu))
+    statistics in eval mode), followed by the activation `act` (None, "relu" or "relu6") -- 3 streaming kernels forward,
+    3 backward.  `relu=True` is the older spelling of act="relu" that the ResNet / DenseNet callers use."""
+    if relu and act not in (None, "relu"):
+        raise ValueError("bn_act: relu=True contradicts act=%r" % (act,))
+    return _BnAct.apply(x, bn.weight, bn.bias, bn, ACT_CODES["relu" if relu else act])
 
 
 # ------------------------------------------------------------------------------------------------ BN -> ReLU -> conv
@@ -355,3 +366,125 @@ class _BnAddRelu(torch.autograd.Function):
 def bn_add_relu(x, res, bn):
     """relu(bn(x) + res): the tail of a torchvision Bottleneck, one streaming kernel after the statistics"""
     return _BnAddRelu.apply(x, res, bn.weight, bn.bias, bn)
+
+
+# ------------------------------------------------------------------------------------------------ MobileNetV2 glue
+def _bn_apply(x, st, act, res=None):
+    """act(x*st[0] + st[1]) [+ res] into a fresh NHWC tensor (bts_bn_apply / bts_bn_add)"""
+    x, xs = _nhwc(x)
+    B, C, H, W = x.shape
+    y = _new(B, C, H, W, x.device)
+    L = _lib.lib()
+    if res is None:
+        _lib.check(L.bts_bn_apply(_ptr(x), xs, B * H * W, C, _ptr(st[0]), _ptr(st[1]), int(act), _ptr(y), C, _stream()),
+                   "bts_bn_apply")
+    else:
+        r, rs = _nhwc(res)
+        _lib.check(L.bts_bn_add(_ptr(x), xs, B * H * W, C, _ptr(st[0]), _ptr(st[1]), _ptr(r), rs, _ptr(y), C, _stream()),
+                   "bts_bn_add")
+    _lib.count()
+    return y
+
+
+def _stats_buffer(C, dev):
+    return torch.zeros((2, C), device=dev, dtype=torch.float64)
+
+
+class _InvertedResidual(torch.autograd.Function):
+    """torchvision InvertedResidual [1x1 -> BN1 -> ReLU6 ->] dw 3x3 -> BN2 -> ReLU6 -> 1x1 -> BN3 [+ x]"""
+
+    @staticmethod
+    def forward(ctx, x, w1, g1, b1, w2, g2, b2, w3, g3, b3, bns, stride, res, fuse_eval):
+        from . import dwconv
+        bn1, bn2, bn3 = bns
+        x, _ = _nhwc(x)
+        B, _, H, W = x.shape
+        Ho, Wo = (H - 1) // stride + 1, (W - 1) // stride + 1
+        y1 = st1 = pre = None
+        t1 = False
+        if w1 is not None:                          # expand 1x1 on the engine, BN1 statistics from its epilogue
+            t1 = bn_uses_batch_stats(bn1)
+            s1 = _stats_buffer(w1.shape[0], x.device) if t1 else None
+            y1 = conv.conv2d_tc(x, w1, stats=s1)
+            st1 = bn_finalize(s1, B * H * W, bn1, g1, b1, t1)
+            pre = (st1[0], st1[1])
+        dw_in = x if y1 is None else y1
+        t2 = bn_uses_batch_stats(bn2)
+        y2 = None
+        if t2:                                      # depthwise with the BN1 + ReLU6 prologue and BN2 statistics epilogue
+            y2, s2 = dwconv.fwd(dw_in, w2, stride, pre=pre, stats=True)
+            st2 = bn_finalize(s2, B * Ho * Wo, bn2, g2, b2, True)
+            a2 = _bn_apply(y2, st2, 2)
+        else:
+            st2 = bn_finalize(None, B * Ho * Wo, bn2, g2, b2, False)
+            if fuse_eval:                           # no backward follows: relu6(bn2(.)) from the folded statistics
+                a2 = dwconv.fwd(dw_in, w2, stride, pre=pre, post=(st2[0], st2[1]))   # in the epilogue
+            else:                                   # the backward needs the BN2 input y2
+                y2 = dwconv.fwd(dw_in, w2, stride, pre=pre)
+                a2 = _bn_apply(y2, st2, 2)
+        t3 = bn_uses_batch_stats(bn3)
+        s3 = _stats_buffer(w3.shape[0], x.device) if t3 else None
+        y3 = conv.conv2d_tc(a2, w3, stats=s3)
+        st3 = bn_finalize(s3, B * Ho * Wo, bn3, g3, b3, t3)
+        out = _bn_apply(y3, st3, 0, x if res else None)
+        ctx.cfg = (stride, res, t1, t2, t3, H, W)
+        ctx.save_for_backward(x, w1, w2, w3, y1, st1, y2, st2, a2, y3, st3)
+        return out
+
+    @staticmethod
+    def backward(ctx, gy):
+        from . import dwconv
+        x, w1, w2, w3, y1, st1, y2, st2, a2, y3, st3 = ctx.saved_tensors
+        stride, res, t1, t2, t3, H, W = ctx.cfg
+        need = ctx.needs_input_grad
+        g, _ = _nhwc(gy)
+        gx = gw1 = gw2 = gw3 = G1 = G2 = G3 = None
+        need_a1 = need[0] or any(need[1:4])               # the gradient has to reach the depthwise input
+        need_y2 = need_a1 or any(need[4:7])
+        g_y3, G3 = bn_backward(y3, g, st3, t3, 0)
+        if need[7]:
+            gw3 = conv.wgrad_tc(a2, g_y3, w3.shape, w3.stride())
+        if need_y2:
+            g_a2 = conv.conv2d_tc(g_y3, w3, 1, 0, 1, transpose_flip=True)
+            g_y2, G2 = bn_backward(y2, g_a2, st2, t2, 2, out=g_a2)
+            dw_in = x if y1 is None else y1
+            pre = None if st1 is None else (st1[0], st1[1])
+            if need[4]:
+                gw2 = dwconv.wgrad(dw_in, g_y2, w2, stride, pre=pre)
+            if need_a1:
+                g_a1 = dwconv.dgrad(g_y2, w2, stride, H, W)
+                if w1 is None:
+                    gx = g_a1
+                else:
+                    g_y1, G1 = bn_backward(y1, g_a1, st1, t1, 2, out=g_a1)
+                    if need[1]:
+                        gw1 = conv.wgrad_tc(x, g_y1, w1.shape, w1.stride())
+                    if need[0]:
+                        gx = conv.conv2d_tc(g_y1, w1, 1, 0, 1, transpose_flip=True)
+        if need[0] and res:
+            if gx is None:
+                gx = g.clone(memory_format=torch.channels_last)
+            else:
+                copy_channels(g, gx, accumulate=True)     # residual branch: dx += dy
+        dg = lambda G, i: G[1].float() if need[i] and G is not None else None
+        db = lambda G, i: G[0].float() if need[i] and G is not None else None
+        return (gx if need[0] else None, gw1, dg(G1, 2), db(G1, 3), gw2, dg(G2, 5), db(G2, 6), gw3, dg(G3, 8), db(G3, 9),
+                None, None, None, None)
+
+
+def inverted_residual(x, block):
+    """torchvision InvertedResidual `block` (re-classed by model.adopt_convs) applied to x as one autograd Function"""
+    layers = list(block.conv)
+    if len(layers) == 4:
+        expand, dw, proj, bn3 = layers
+        w1, g1, b1, bn1 = expand[0].weight, expand[1].weight, expand[1].bias, expand[1]
+    else:
+        dw, proj, bn3 = layers
+        w1 = g1 = b1 = bn1 = None
+    bn2 = dw[1]
+    # BN2 on folded running statistics can run as the depthwise conv's epilogue only when no backward follows.  That is
+    # decided here: inside the Function, needs_input_grad reflects requires_grad alone and ignores no_grad / inference_mode.
+    fuse_eval = not bn_uses_batch_stats(bn2) and not (
+        torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in block.parameters())))
+    return _InvertedResidual.apply(x, w1, g1, b1, dw[0].weight, bn2.weight, bn2.bias, proj.weight, bn3.weight, bn3.bias,
+                                   (bn1, bn2, bn3), int(dw[0].stride[0]), bool(block.use_res_connect), fuse_eval)

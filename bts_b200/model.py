@@ -67,6 +67,10 @@ class Conv2dTC(nn.Conv2d):
                 if conv.c1_eligible(self.weight, self.stride[0], self.padding[0], self.dilation[0]):
                     return conv.conv_c1(x, self.weight, sigmoid=False)
                 return conv.conv2d(x, self.weight, self.stride[0], self.padding[0], self.dilation[0])
+            from . import dwconv
+            if dwconv.eligible(self):
+                # depthwise 3x3 (MobileNetV2): CUDA-core kernels, fwd / dgrad / wgrad
+                return dwconv.conv(x, self.weight, self.stride[0])
             cpg = self.in_channels // self.groups
             if (self.in_channels == self.out_channels and cpg >= 4 and conv.group_window(self.out_channels, cpg) == 128):
                 # ResNeXt grouped 3x3 (32 groups): block-diagonal operator on the engine, fwd / dgrad / wgrad
@@ -174,14 +178,69 @@ def _dense_block_class():
     return _DenseBlock, DenseBlockTC
 
 
+def _mobilenet_classes():
+    from torchvision.models.mobilenetv2 import InvertedResidual
+    from torchvision.ops.misc import Conv2dNormActivation
+
+    class InvertedResidualTC(InvertedResidual):
+        """torchvision MobileNetV2 block [1x1 -> BN -> ReLU6 ->] depthwise 3x3 -> BN -> ReLU6 -> 1x1 -> BN [+ x] as one
+        autograd Function (glue.inverted_residual): 1x1 convs on the wgmma engine, the depthwise conv on the CUDA-core
+        kernels with the BatchNorm + ReLU6 in front of it folded into its prologue, BN statistics from the epilogues;
+        parameters / buffers / state_dict untouched."""
+
+        def forward(self, x):
+            from . import glue
+            if fuse_enabled(x) and _inverted_residual_eligible(self):
+                return glue.inverted_residual(x, self)
+            return super().forward(x)
+
+    class ConvNormReLU6TC(Conv2dNormActivation):
+        """torchvision Conv2dNormActivation(conv, BN, ReLU6) -- mobilenet_v2's 3x3/2 stem and its last 1x1: the conv on the
+        engine, BN + ReLU6 on the streaming kernels"""
+
+        def forward(self, x):
+            if fuse_enabled(x) and len(self) == 3 and isinstance(self[1], nn.BatchNorm2d) and self[1].affine \
+                    and type(self[2]) is nn.ReLU6:
+                from . import glue
+                return glue.bn_act(self[0](x), self[1], act="relu6")
+            return super().forward(x)
+
+    return InvertedResidual, InvertedResidualTC, Conv2dNormActivation, ConvNormReLU6TC
+
+
+def _inverted_residual_eligible(block):
+    """the layer sequence the fused block Function implements (torchvision's, expand ratio 1 or > 1)"""
+    from . import dwconv
+    layers = list(block.conv)
+    cnas = layers[:-2]
+    if len(cnas) not in (1, 2) or not isinstance(layers[-2], nn.Conv2d) or not isinstance(layers[-1], nn.BatchNorm2d):
+        return False
+    for cna in cnas:
+        if len(cna) != 3 or not isinstance(cna[1], nn.BatchNorm2d) or not cna[1].affine or type(cna[2]) is not nn.ReLU6 \
+                or cna[0].bias is not None:
+            return False
+    if len(cnas) == 2 and (tuple(cnas[0][0].kernel_size) != (1, 1) or cnas[0][0].groups != 1 or cnas[0][0].stride != (1, 1)):
+        return False
+    proj = layers[-2]
+    return (dwconv.eligible(cnas[-1][0]) and tuple(proj.kernel_size) == (1, 1) and proj.groups == 1 and proj.bias is None
+            and proj.stride == (1, 1) and layers[-1].affine)
+
+
 def adopt_convs(module):
-    """Re-class every eligible nn.Conv2d (-> Conv2dTC) and DenseNet block (-> fused DenseBlockTC) of a torchvision
-    module tree in place -- parameter names, shapes and init are untouched."""
+    """Re-class every eligible nn.Conv2d (-> Conv2dTC), DenseNet block (-> fused DenseBlockTC), ResNet bottleneck and
+    MobileNetV2 block / conv-norm-activation of a torchvision module tree in place -- parameter names, shapes and init
+    are untouched."""
     base, fusedcls = _dense_block_class()
     tbase, tcls = _transition_class()
     bbase, bcls = _bottleneck_class()
+    ibase, icls, cbase, ccls = _mobilenet_classes()
     resnet = any(type(m) is bbase for m in module.modules())
+    in_blocks = {id(m) for b in module.modules() if type(b) is ibase for m in b.modules()}
     for m in module.modules():
+        if type(m) is ibase:
+            m.__class__ = icls
+        elif type(m) is cbase and id(m) not in in_blocks:
+            m.__class__ = ccls                 # mobilenet_v2 features[0] (stem) and features[18]
         if type(m) is nn.Conv2d:
             m.__class__ = Conv2dTC
         elif type(m) is base:

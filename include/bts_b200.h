@@ -217,13 +217,15 @@ int bts_bn_relu_bwd_apply(const float *x, long long x_pixel_stride, const float 
                           long long M, int C, const float *scale, const float *shift, const float *coef, float *out,
                           long long out_pixel_stride, int accumulate, void *stream);
 
-/* generalised forms with an explicit `relu` flag (relu=0: plain BatchNorm, as the decoder's bn5/bn4/bn4_2/bn3/bn2 which
- * feed a concat, bts.py:200-246); the *_relu_* entry points above are these with relu=1. */
+/* generalised forms with an explicit activation code `act`: 0 none (plain BatchNorm, as the decoder's bn5/bn4/bn4_2/bn3/bn2
+ * which feed a concat, bts.py:200-246), 1 ReLU, 2 ReLU6 (torchvision mobilenet_v2's Conv2dNormActivation / InvertedResidual,
+ * bts.py:297-300; its backward mask is 0 < y < 6, strictly, as hardtanh_backward); the *_relu_* entry points above are these
+ * with act=1. */
 int bts_bn_bwd_reduce(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride, long long M,
-                      int C, const float *scale, const float *shift, const float *mean, const float *invstd, int relu,
+                      int C, const float *scale, const float *shift, const float *mean, const float *invstd, int act,
                       double *S1, double *S2, float *coef, void *stream);
 int bts_bn_bwd_apply(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride, long long M,
-                     int C, const float *scale, const float *shift, const float *coef, int relu, float *out,
+                     int C, const float *scale, const float *shift, const float *coef, int act, float *out,
                      long long out_pixel_stride, int accumulate, void *stream);
 
 /* One-pass BatchNorm+ReLU backward into a concat gradient slab (the dense-block fan-out, torchvision densenet.py
@@ -239,8 +241,9 @@ int bts_bn_bwd_correct(const float *x, long long x_pixel_stride, long long M, in
 
 /* ---- streaming NHWC glue kernels of the decoder / encoder transitions (csrc/elem.cu) ---------------------------
  * All take explicit pixel strides (floats) so channel slices of wider slabs are read / written in place.
- *   bts_bn_apply       out = x*scale + shift [, ReLU]   -- BatchNorm2d forward given (scale, shift) from bts_bn_finalize /
- *                      bts_bn_fold (decoder BNs bts.py:154-182; torchvision norm0 / norm5)
+ *   bts_bn_apply       out = act(x*scale + shift)       -- BatchNorm2d forward given (scale, shift) from bts_bn_finalize /
+ *                      bts_bn_fold (decoder BNs bts.py:154-182; torchvision norm0 / norm5); `act` is the activation code
+ *                      0 none, 1 ReLU, 2 ReLU6 (min(max(y, 0), 6): mobilenet_v2's BN + ReLU6 pairs)
  *   bts_elu_bwd        out = gy * (y > 0 ? 1 : y + 1)   -- backward of nn.ELU() through its saved OUTPUT y (bts.py:72,79,...)
  *   bts_upsample2_sum  out[b,y,x,:] = sum of g[b,2y..2y+1,2x..2x+1,:]  -- backward of F.interpolate(scale_factor=2,
  *                      mode='nearest') (bts.py:77); relu_src != NULL additionally gates by relu_src > 0 (torch.nn.ReLU in
@@ -249,7 +252,7 @@ int bts_bn_bwd_correct(const float *x, long long x_pixel_stride, long long M, in
  *   bts_zero_channels  dst[:, c0:c1] = 0                -- alignment padding channels of concat3 (225) / concat2 (161)
  *   bts_avgpool2_fwd/bwd  2x2 stride-2 average pooling of the DenseNet transitions (torchvision densenet.py `pool`) */
 int bts_bn_apply(const float *x, long long x_pixel_stride, long long M, int C, const float *scale, const float *shift,
-                 int relu, float *out, long long out_pixel_stride, void *stream);
+                 int act, float *out, long long out_pixel_stride, void *stream);
 int bts_elu_bwd(const float *gy, long long gy_pixel_stride, const float *y, long long y_pixel_stride, long long M, int C,
                 float *out, long long out_pixel_stride, void *stream);
 int bts_upsample2_sum(const float *g, long long g_pixel_stride, int B, int H, int W, int C, const float *relu_src,
@@ -278,17 +281,51 @@ int bts_conv_pw_wgrad(const float *x, long long x_pixel_stride, const float *dy,
 
 /* ResNet / ResNeXt encoder glue (torchvision.models.resnet behind reference pytorch/bts.py:282-296):
  *   bts_bn_add_relu   out = max(x*scale + shift + res, 0)            Bottleneck tail  relu(bn3(conv3(.)) + identity)
+ *   bts_bn_add        out = x*scale + shift + res                    MobileNetV2 inverted-residual tail x + bn3(conv3(.))
+ *                                                                    (torchvision InvertedResidual, use_res_connect)
  *   bts_relu_bwd      out = gy * (y > 0)                             its backward (through the saved output y)
  *   bts_maxpool3s2_*  3x3 / stride 2 / pad 1 max-pool (the encoder stems' pool0 / maxpool), NHWC; forward records the
  *                     winning window position (uint8 per OUTPUT element, dense [B,Ho,Wo,C]) -> deterministic gather backward */
 int bts_bn_add_relu(const float *x, long long x_pixel_stride, long long M, int C, const float *scale, const float *shift,
                     const float *res, long long res_pixel_stride, float *out, long long out_pixel_stride, void *stream);
+int bts_bn_add(const float *x, long long x_pixel_stride, long long M, int C, const float *scale, const float *shift,
+               const float *res, long long res_pixel_stride, float *out, long long out_pixel_stride, void *stream);
 int bts_relu_bwd(const float *gy, long long gy_pixel_stride, const float *y, long long y_pixel_stride, long long M, int C,
                  float *out, long long out_pixel_stride, void *stream);
 int bts_maxpool3s2_fwd(const float *x, long long x_pixel_stride, int B, int H, int W, int C, float *out,
                        long long out_pixel_stride, unsigned char *argmax, void *stream);
 int bts_maxpool3s2_bwd(const float *g, long long g_pixel_stride, const unsigned char *argmax, int B, int H, int W, int C,
                        float *gx, long long gx_pixel_stride, void *stream);
+
+/* ---- depthwise 3x3 convolution of the MobileNetV2 inverted-residual blocks (csrc/dwconv.cu; torchvision mobilenet_v2
+ * features[1..17] `conv.*` groups == C layer behind reference pytorch/bts.py:297-300, replacing cuDNN's depthwise
+ * forward / backward-data / backward-filter).  NHWC fp32, pad 1, stride 1 or 2, no bias, C % 4 == 0, H x W the INPUT size,
+ * output (H-1)/stride+1 x (W-1)/stride+1.  x, y, dy, dx: 16-byte aligned with pixel strides that are multiples of 4 (channel
+ * slices of wider slabs work).  w: the (C,1,3,3) parameter read in place through its (c, kh, kw) strides.  Anything else
+ * returns BTS_EINVAL before any launch.
+ *   bts_dw3x3_fwd    y = dw(pre(x)) [-> relu6(y*post_scale + post_shift)]
+ *                    pre: relu6(x*pre_scale + pre_shift) per channel (both NULL to skip), applied once per staged element;
+ *                    the zero padding is applied after it.  post: the eval-mode epilogue relu6(bn2(y)) from folded running
+ *                    statistics (both NULL to skip).  stat_sum / stat_sumsq (both or neither; not with post): fp64 per-channel
+ *                    sum and sum of squares of y, WRITTEN (no zeroing needed), reduced deterministically through
+ *                    `workspace` = bts_dw3x3_fwd_workspace_floats(...) floats (8-byte aligned).
+ *   bts_dw3x3_dgrad  dx from dy (dy is (B, Ho, Wo, C)); stride 1 is the forward over flipped taps, stride 2 gathers only the
+ *                    taps that land.
+ *   bts_dw3x3_wgrad  dw[c,kh,kw] = sum_p dy[p,c] * pre(x)[p*stride + (kh,kw) - 1, c], the same optional prologue recomputed
+ *                    from the raw x; per-CTA fp64 partials in `workspace` = bts_dw3x3_wgrad_workspace_floats(...) floats,
+ *                    summed in a fixed order by a second kernel (bit-reproducible).  dw written through its strides.
+ * The *_workspace_floats queries return BTS_EINVAL for shapes the kernels do not take. */
+long long bts_dw3x3_fwd_workspace_floats(int B, int H, int W, int C, int stride);
+int bts_dw3x3_fwd(const float *x, long long x_pixel_stride, int B, int H, int W, int C, int stride, const float *w, long long s_c,
+                  long long s_kh, long long s_kw, const float *pre_scale, const float *pre_shift, const float *post_scale,
+                  const float *post_shift, float *y, long long y_pixel_stride, double *stat_sum, double *stat_sumsq,
+                  float *workspace, void *stream);
+int bts_dw3x3_dgrad(const float *dy, long long dy_pixel_stride, int B, int H, int W, int C, int stride, const float *w,
+                    long long s_c, long long s_kh, long long s_kw, float *dx, long long dx_pixel_stride, void *stream);
+long long bts_dw3x3_wgrad_workspace_floats(int B, int H, int W, int C, int stride);
+int bts_dw3x3_wgrad(const float *x, long long x_pixel_stride, const float *dy, long long dy_pixel_stride, int B, int H, int W,
+                    int C, int stride, const float *pre_scale, const float *pre_shift, float *workspace, float *dw,
+                    long long s_c, long long s_kh, long long s_kw, void *stream);
 
 /* ---- optimizer step of the training loop (reference pytorch/bts_main.py:371-373 torch.optim.AdamW, two groups, eps 1e-3;
  * :456-460 poly LR) as ONE multi-tensor kernel, csrc/optim.cu.  ptrs: device int64 [4n] = param | grad | exp_avg | exp_avg_sq
