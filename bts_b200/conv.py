@@ -183,7 +183,8 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
     """Runs the engine.  x: (B,Cin,Hs,Ws) NHWC-in-memory fp32 CUDA.  Returns (B,Cout,Hout,Wout) channels_last.
     `out` may be a pre-allocated channels_last tensor or a channel slice of one (concat-free writes).
     `stats`: a ZEROED fp64 [2, Cout] tensor that receives per-channel (sum, sum of squares) of the output, reduced in the
-    conv epilogue (Cout <= 256) -- the BatchNorm batch statistics of the tensor being produced.
+    conv epilogue (any Cout: the partials are flushed per n-tile) -- the BatchNorm batch statistics of the tensor being
+    produced.
     `bn_bwd=(x_bn, st, relu)` (with a zeroed `stats`): the output is the gradient w.r.t. [relu](bn(x_bn)); the epilogue also
     reduces the BatchNorm-backward sums S1 = sum g*mask, S2 = sum g*mask*xhat into stats[0], stats[1] (st = [4,C] from
     bn_finalize) -- the separate reduce pass over (x, g) disappears.

@@ -110,7 +110,7 @@ int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws
                  long long out_pixel_stride, int act, int precision, void *stream);
 
 /* bts_conv_fwd that also returns the BatchNorm batch statistics of its output: stat_sum[co] += sum_p out[p,co],
- * stat_sumsq[co] += sum_p out[p,co]^2 (fp64, accumulated with atomics -> zero them first; Cout <= 256, act must be 0).  Replaces a separate
+ * stat_sumsq[co] += sum_p out[p,co]^2 (fp64, accumulated with atomics -> zero them first; any Cout, act must be 0).  Replaces a separate
  * bts_bn_stats pass over the tensor just written (torchvision _DenseLayer: conv1 -> norm2, conv2 -> every later norm1). */
 int bts_conv_fwd_stats(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
                        int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,

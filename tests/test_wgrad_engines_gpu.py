@@ -10,18 +10,19 @@ reduces stay at or below about 2k, where 3xTF32 meets the bar without the K-leng
 tensor cores' fp32 accumulator truncates on every step, and one CTA reducing 3256 pixels of ReLU'd activations (the split
 case below at split 1, on a 2x37x44 map) measured 2.3e-5 on an H100."""
 import ctypes
-import re
+import os
 
 import pytest
 import torch
 import torch.nn.functional as F
+
+from engine_checks import check_written, guarded, kernels, nan, nhwc_slice, ran
 
 pytestmark = pytest.mark.gpu
 
 TOL = 2e-5
 KP = 32                 # pixels per k-block of wgrad_tc_kernel
 SPLIT_PX = 16           # split-K ranges of wgrad2_tc_kernel are whole multiples of this many pixels
-GUARD = 64              # NaN floats on each side of the dW view
 
 
 def _L():
@@ -33,6 +34,12 @@ def _route(tap_in_grid, tma=1):
     L = _L()
     L.bts_wgrad2_set_min_pixels(1 << 40 if tap_in_grid else 0)
     L.bts_wgrad2_set_tma(tma)
+
+
+def _capped_grid():
+    """BTS_B200_SM_LIMIT (read with atoi by csrc/util.cu) caps the library's grids below this GPU's SM count"""
+    lim = int(os.environ.get("BTS_B200_SM_LIMIT") or 0)
+    return 0 < lim < torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
 
 
 def _restore():
@@ -66,44 +73,6 @@ def route(request):
 
 
 # --------------------------------------------------------------------------------------------------------------- helpers
-def _template_arg(a):
-    a = re.sub(r"^\((int|bool)\)", "", a.strip())           # '(bool)1' / 'true' / '1', whichever demangler named it
-    return {"true": 1, "false": 0}[a] if a in ("true", "false") else int(a)
-
-
-def _kernels(prof):
-    """(name, template arguments as ints) of every wgrad kernel the profiled region launched"""
-    out = []
-    for e in prof.events():
-        m = re.search(r"(wgrad2?_tc_kernel)<([^<>]*)>", e.name)
-        if m:
-            out.append((m.group(1), tuple(_template_arg(a) for a in m.group(2).split(","))))
-            continue
-        m = re.search(r"(wgrad2?_tc_kernel)I((?:L[ib]\d+E)+)E", e.name)       # a name left mangled
-        if m:
-            out.append((m.group(1), tuple(int(a) for a in re.findall(r"L[ib](\d+)E", m.group(2)))))
-    return out
-
-
-def _nan(n):
-    return torch.full((n,), float("nan"), device="cuda")
-
-
-def _guarded(shape, strides):
-    """a NaN-filled view of `shape` with `strides` inside a larger NaN-filled buffer: (view, buffer, membership mask)"""
-    extent = 1 + sum((n - 1) * s for n, s in zip(shape, strides))
-    buf = _nan(extent + 2 * GUARD)
-    inside = torch.zeros(buf.numel(), dtype=torch.bool, device="cuda")
-    inside.as_strided(shape, strides, GUARD).fill_(True)
-    assert int(inside.sum()) == torch.Size(shape).numel()          # the layout does not alias
-    return buf.as_strided(shape, strides, GUARD), buf, inside
-
-
-def _check_written(dw, buf, inside):
-    assert bool(torch.isfinite(dw).all()), "dW has %d non-finite elements" % int((~torch.isfinite(dw)).sum())
-    assert bool(torch.isnan(buf[~inside]).all()), "a write landed outside the dW view"
-
-
 def _weight_strides(Cout, Cin, k, layout):
     if layout == "contiguous":
         return (Cin * k * k, k * k, k, 1)
@@ -140,9 +109,9 @@ def wgrad(x, gy, k, stride=1, pad=0, dil=1, scale=None, shift=None, relu=False, 
                    "bts_conv_wgrad_plan")
         split = sp.value
         assert wsf.value == split * k * k * Cin * Cout
-    ws = _nan(split * k * k * Cin * Cout)
+    ws = nan(split * k * k * Cin * Cout)
     s = _weight_strides(Cout, Cin, k, layout)
-    dw, buf, inside = _guarded((Cout, Cin, k, k), s)
+    dw, buf, inside = guarded((Cout, Cin, k, k), s)
     torch.cuda.synchronize()
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         rc = L.bts_conv_wgrad(_ptr(x), xs, B, Hs, Ws, int(up), Cin, k, k, stride, pad, dil, _ptr(scale), _ptr(shift),
@@ -150,19 +119,8 @@ def wgrad(x, gy, k, stride=1, pad=0, dil=1, scale=None, shift=None, relu=False, 
                               int(precision), _stream())
         _lib.check(rc, "bts_conv_wgrad")
         torch.cuda.synchronize()
-    _check_written(dw, buf, inside)
-    return dw, split, _kernels(prof)
-
-
-def _dev(t, width=None, off=0):
-    """t on the GPU, NHWC in memory, as the channel slice [off, off + C) of a slab `width` channels wide (other channels
-    hold unrelated values)"""
-    B, C, H, W = t.shape
-    width = C if width is None else width
-    slab = torch.randn(B, width, H, W).cuda().contiguous(memory_format=torch.channels_last)
-    v = slab[:, off:off + C]
-    v.copy_(t)
-    return v
+    check_written(dw, buf, inside)
+    return dw, split, kernels(prof)
 
 
 class Case:
@@ -190,22 +148,13 @@ class Case:
         self.ref = wd.grad
 
     def run(self, x_width=None, x_off=0, dy_width=None, dy_off=0, **kw):
-        x, gy = _dev(self.x, x_width, x_off), _dev(self.gy, dy_width, dy_off)
+        x, gy = nhwc_slice(self.x, x_width, x_off), nhwc_slice(self.gy, dy_width, dy_off)
         sc = self.scale.cuda() if self.scale is not None else None
         sh = self.shift.cuda() if self.shift is not None else None
         return wgrad(x, gy, self.k, self.stride, self.pad, self.dil, sc, sh, bool(self.pre & 1), self.up, **kw)
 
     def err(self, dw):
         return float((dw.detach().cpu().double() - self.ref).abs().max() / self.ref.abs().max())
-
-
-def _ran(kernels, name, args=()):
-    """the profiled call launched `name` (and not the other wgrad kernel) with template arguments starting with `args`.
-    CUPTI now and then delivers no kernel record for a profiled region this short; there is then nothing to compare,
-    and the numerical checks of the test stand alone."""
-    if not kernels:
-        return True
-    return [n for n, _ in kernels] == [name] and kernels[0][1][:len(args)] == tuple(int(a) for a in args)
 
 
 # ------------------------------------------------------------------------------------------- tap-in-grid kernel (wgrad_tc)
@@ -221,7 +170,7 @@ def test_tap_in_grid_every_instantiation(tap_in_grid, pre, up, load):
     c = Case(2, 70, 6, 9, 72, 3, pre=pre, up=up, seed=100 + 10 * pre + up)
     kw = {"vec": dict(x_width=72), "x_stride": dict(x_width=71), "dy_offset": dict(x_width=72, dy_width=76, dy_off=1)}[load]
     dw, _, ks = c.run(**kw)
-    assert _ran(ks, "wgrad_tc_kernel", (pre, up, load == "vec")), ks
+    assert ran(ks, "wgrad_tc_kernel", (pre, up, load == "vec")), ks
     assert c.err(dw) < TOL
 
 
@@ -233,7 +182,7 @@ def test_tap_in_grid_output_tile_widths(tap_in_grid, Cout, k):
     tiles; the 1x1 layer with Cout = 1056 runs 17 tiles of 64, the last one half live"""
     c = Case(1, 40, 9, 13, Cout, k, seed=Cout + k)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad_tc_kernel", (0, False, True)), ks
+    assert ran(ks, "wgrad_tc_kernel", (0, False, True)), ks
     assert c.err(dw) < TOL
 
 
@@ -259,7 +208,7 @@ def test_tap_in_grid_decoder_layers(tap_in_grid, name, B, Cin, Hs, Ws, Cout, dil
     Cin (scalar loads).  conv2 runs on the shifted-dY kernel in production; here it is forced onto this one."""
     c = Case(B, Cin, Hs, Ws, Cout, 3, dil=dil, pre=pre, up=up, seed=Cin + Cout + dil)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad_tc_kernel", (pre, up, Cin % 4 == 0)), ks
+    assert ran(ks, "wgrad_tc_kernel", (pre, up, Cin % 4 == 0)), ks
     assert c.err(dw) < TOL
 
 
@@ -269,7 +218,7 @@ def test_tap_in_grid_stride2(tap_in_grid, B, Cin, H, W, Cout, k, pad):
     stem with Cin = 3 (49 taps in the grid, one partial 4-channel unit, scalar loads)"""
     c = Case(B, Cin, H, W, Cout, k, stride=2, pad=pad, seed=k + Cin)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad_tc_kernel", (0,)), ks
+    assert ran(ks, "wgrad_tc_kernel", (0,)), ks
     assert c.err(dw) < TOL
 
 
@@ -279,7 +228,7 @@ def test_tap_in_grid_padding_not_same(tap_in_grid, pad, dil):
     pad > dil leaves output rows whose every tap but one reads padding"""
     c = Case(2, 48, 10, 13, 40, 3, pad=pad, dil=dil, pre=3, seed=pad + 10 * dil)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad_tc_kernel", (3, False, True)), ks
+    assert ran(ks, "wgrad_tc_kernel", (3, False, True)), ks
     assert c.err(dw) < TOL
 
 
@@ -294,7 +243,7 @@ def test_tap_in_grid_forced_split(tap_in_grid, split):
     (as zeros) into the NaN-filled workspace.  A split-K result is bit-reproducible: fixed summation order."""
     c = Case(**SPLIT_CASE, pre=3, seed=7)
     dw, sp, ks = c.run(split=split)
-    assert sp == split and _ran(ks, "wgrad_tc_kernel", (3, False, True)), ks
+    assert sp == split and ran(ks, "wgrad_tc_kernel", (3, False, True)), ks
     assert c.err(dw) < TOL
     if split > 1:
         dw2, _, _ = c.run(split=split)
@@ -316,7 +265,7 @@ def test_precision_flag_reaches_both_kernels(route):
     d3, _, ks = c.run()
     d1, _, ks1 = c.run(precision=1)
     name = "wgrad_tc_kernel" if route == "tap_in_grid" else "wgrad2_tc_kernel"
-    assert _ran(ks, name) and _ran(ks1, name), ks
+    assert ran(ks, name) and ran(ks1, name), ks
     e3, e1 = c.err(d3), c.err(d1)
     assert e3 < TOL and 1e-5 < e1 < 5e-3, (e3, e1)
 
@@ -324,17 +273,21 @@ def test_precision_flag_reaches_both_kernels(route):
 @pytest.mark.parametrize("k,Cout", [(3, 48), (3, 512), (1, 136)])
 def test_production_wgrad_matches_explicit_split_bitwise(route, k, Cout):
     """conv.wgrad_tc (the plan's split, torch.empty workspace) and the explicit-split ABI call at that split give
-    bit-identical dW, on whichever kernel the routing picks; 4096 output pixels so the plan splits the reduction"""
+    bit-identical dW, on whichever kernel the routing picks; 4096 output pixels so the plan splits the reduction on the
+    full grid.  On a grid capped by BTS_B200_SM_LIMIT the plan may keep one split, and one CTA reducing all 4096 pixels
+    is past the ~2k where 3xTF32 meets the bar (see above): there the claim is bit-identity alone."""
     from bts_b200 import conv
     c = Case(1, 64, 64, 64, Cout, k, seed=k * Cout)
     dw, sp, ks = c.run()
-    assert c.err(dw) < TOL
-    x, gy = _dev(c.x), _dev(c.gy)
+    assert sp > 1 or _capped_grid()
+    if sp > 1:
+        assert c.err(dw) < TOL
+    x, gy = nhwc_slice(c.x), nhwc_slice(c.gy)
     gw = conv.wgrad_tc(x, gy, (Cout, 64, k, k), (64 * k * k, k * k, k, 1), 1, c.pad, 1)
     torch.cuda.synchronize()
     assert torch.equal(gw, dw)
     if route == "tap_in_grid":
-        assert sp > 1 and _ran(ks, "wgrad_tc_kernel")
+        assert ran(ks, "wgrad_tc_kernel")
 
 
 # ---------------------------------------------------------------------------------------- shifted-dY kernel (wgrad2_tc)
@@ -346,7 +299,7 @@ def test_shifted_dy_pre_ops(shifted_dy, pre, up):
     third 16-channel co-group half live, Cin = 72 a partial 64-channel tile"""
     c = Case(2, 72, 7, 10, 40, 3, pre=pre, up=up, seed=200 + 10 * pre + up)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad2_tc_kernel", (pre, up, True, shifted_dy == "tma_ring")), ks
+    assert ran(ks, "wgrad2_tc_kernel", (pre, up, True, shifted_dy == "tma_ring")), ks
     assert c.err(dw) < TOL
 
 
@@ -356,7 +309,7 @@ def test_shifted_dy_unaligned_dy_slice(shifted_dy, pre):
     false) runs even where the TMA ring is enabled"""
     c = Case(2, 36, 9, 12, 32, 3, pre=pre, seed=300 + pre)
     dw, _, ks = c.run(dy_width=36, dy_off=1)
-    assert _ran(ks, "wgrad2_tc_kernel", (pre, False, False, False)), ks
+    assert ran(ks, "wgrad2_tc_kernel", (pre, False, False, False)), ks
     assert c.err(dw) < TOL
 
 
@@ -366,7 +319,7 @@ def test_shifted_dy_pointwise_uneven_co_groups(shifted_dy, Cout):
     two groups of 80 / 56 live channels, 250 two 128-wide groups, the second with 122 live (odd Cout: scalar dY loads)"""
     c = Case(2, 100, 8, 11, Cout, 1, pre=3, seed=Cout)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad2_tc_kernel", (3,)), ks
+    assert ran(ks, "wgrad2_tc_kernel", (3,)), ks
     assert c.err(dw) < TOL
 
 
@@ -376,7 +329,7 @@ def test_shifted_dy_padding_not_same(shifted_dy, pad):
     input grid onto the output grid, so these shapes skip the landing ring and use the load path"""
     c = Case(2, 64, 11, 13, 48, 3, pad=pad, pre=3, seed=400 + pad)
     dw, _, ks = c.run()
-    assert _ran(ks, "wgrad2_tc_kernel", (3, False, True, False)), ks
+    assert ran(ks, "wgrad2_tc_kernel", (3, False, True, False)), ks
     assert c.err(dw) < TOL
 
 
@@ -387,7 +340,7 @@ def test_shifted_dy_splits_beyond_pixels(shifted_dy, k, Cout, B, H, W):
     c = Case(B, 40, H, W, Cout, k, pre=1, seed=500 + Cout)
     split = -(-B * H * W // SPLIT_PX) + 3
     dw, sp, ks = c.run(split=split)
-    assert sp == split and _ran(ks, "wgrad2_tc_kernel", (1,)), ks
+    assert sp == split and ran(ks, "wgrad2_tc_kernel", (1,)), ks
     assert c.err(dw) < TOL
 
 
@@ -406,15 +359,15 @@ def test_grouped_forced_split_with_empty_splits(split):
     gy = torch.randn(B, width, H, W, generator=g)
     wd = torch.zeros(width, cpg, 3, 3, dtype=torch.float64, requires_grad=True)
     F.conv2d(x.double(), wd, None, 1, 1, 1, width // cpg).backward(gy.double())
-    xc, gc = _dev(x), _dev(gy)
-    ws = _nan(split * 9 * width * 128)
+    xc, gc = nhwc_slice(x), nhwc_slice(gy)
+    ws = nan(split * 9 * width * 128)
     s = (cpg * 9, 9, 3, 1)
-    dw, buf, inside = _guarded((width, cpg, 3, 3), s)
+    dw, buf, inside = guarded((width, cpg, 3, 3), s)
     with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
         rc = L.bts_conv_wgrad_grouped(_ptr(xc), width, B, H, W, width, cpg, 3, 3, 1, 1, 1, _ptr(gc), width, _ptr(ws), split,
                                       _ptr(dw), s[0], s[1], s[2], s[3], 0, _stream())
         _lib.check(rc, "bts_conv_wgrad_grouped")
         torch.cuda.synchronize()
-    assert _ran(_kernels(prof), "wgrad_tc_kernel", (0, False, True))
-    _check_written(dw, buf, inside)
+    assert ran(kernels(prof), "wgrad_tc_kernel", (0, False, True))
+    check_written(dw, buf, inside)
     assert float((dw.cpu().double() - wd.grad).abs().max() / wd.grad.abs().max()) < TOL
