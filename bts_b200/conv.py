@@ -4,6 +4,11 @@ Activations are NHWC in memory: torch tensors of logical shape (B,C,H,W) in `cha
 tensor is understood by the rest of torch (cat, BatchNorm, autograd) without transposes.  Weights keep the
 reference's (Cout,Cin,kh,kw) parameter layout (checkpoint wire format) and are re-packed into the engine's
 pre-split, pre-swizzled tile stream whenever the parameter's version counter changes (i.e. once per optimizer step).
+
+Numeric mode of the tensor-core engine (set_precision / BTS_B200_PRECISION): "fp32" (default) runs every GEMM as 3xTF32,
+fp32-grade; "tf32" runs the single-pass TF32 kernels, one product per MMA.  Only the engine's forward, dgrad and wgrad
+follow the mode; the CUDA-core kernels (narrow 1x1 and Cout = 1 heads, depthwise, BatchNorm, LPG, loss, optimizer) and
+the library-conv fallback compute in fp32 either way, and their routing does not depend on it.
 """
 import ctypes
 import weakref
@@ -21,6 +26,37 @@ PW_WGRAD = True                                               # CUDA-core wgrad 
 PW_MIN_PIXELS = 200000                                        # below this the tensor-core path is already short
 TRACE = _os.environ.get("BTS_B200_TRACE", "0") == "1"     # per-call CUDA-event timing, aggregated by shape
 trace_log = []
+
+
+PRECISIONS = {"fp32": 0, "tf32": 1}       # mode -> the `precision` argument of the C ABI
+
+
+def _check_mode(mode, what):
+    if not isinstance(mode, str) or mode not in PRECISIONS:
+        raise ValueError("%s: unknown precision mode %r (expected one of %s)" % (what, mode, ", ".join(sorted(PRECISIONS))))
+    return mode
+
+
+_precision = _check_mode(_os.environ.get("BTS_B200_PRECISION", "fp32"), "BTS_B200_PRECISION")
+
+
+def set_precision(mode):
+    """Selects the numeric mode of every later tensor-core engine launch -- forward, dgrad and wgrad of the whole model:
+    "fp32" (the default: 3xTF32, fp32-grade) or "tf32" (single-pass TF32: faster, about 1e-3 relative per layer).
+    Returns the previous mode, so that a caller can restore it.  The mode is read when a launch is enqueued: a captured
+    CUDA graph (bts_b200.graph.GraphedTrainStep) keeps replaying the mode it was captured in."""
+    global _precision
+    prev, _precision = _precision, _check_mode(mode, "set_precision")
+    return prev
+
+
+def get_precision():
+    return _precision
+
+
+def _engine_precision(precision):
+    """the C ABI's `precision` of an engine call: explicit 0 / 1, or None = the current mode"""
+    return PRECISIONS[_precision] if precision is None else int(precision)
 
 
 def set_trace(on):
@@ -178,7 +214,7 @@ def _nhwc_view(x):
 
 
 def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_shift=None, pre_relu=False,
-              upsample2=False, act=None, out=None, precision=0, packed=None, cout=None, transpose_flip=False,
+              upsample2=False, act=None, out=None, precision=None, packed=None, cout=None, transpose_flip=False,
               stats=None, groups=1, zero_stuff_out=None, bn_bwd=None):
     """Runs the engine.  x: (B,Cin,Hs,Ws) NHWC-in-memory fp32 CUDA.  Returns (B,Cout,Hout,Wout) channels_last.
     `out` may be a pre-allocated channels_last tensor or a channel slice of one (concat-free writes).
@@ -189,7 +225,9 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
     reduces the BatchNorm-backward sums S1 = sum g*mask, S2 = sum g*mask*xhat into stats[0], stats[1] (st = [4,C] from
     bn_finalize) -- the separate reduce pass over (x, g) disappears.
     `groups` > 1: block-diagonal operator (ResNeXt 3x3).  `zero_stuff_out=(H,W)`: x is the gradient of a stride-2 layer
-    whose input was HxW -- the source is read as its zero-stuffed x2 expansion (use with transpose_flip, stride 1)."""
+    whose input was HxW -- the source is read as its zero-stuffed x2 expansion (use with transpose_flip, stride 1).
+    `precision`: None = the mode of set_precision, 0 = 3xTF32, 1 = single-pass TF32 on the engine (an explicit 1 also
+    keeps the layer off the CUDA-core 1x1 kernel, which is fp32 in every mode)."""
     _need_cuda(x, weight)
     if x.dtype != torch.float32:
         raise TypeError("conv2d_tc computes in fp32 (3xTF32 on wgmma); got %s" % x.dtype)
@@ -208,7 +246,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         raise ValueError("weight expects %d input channels, got %d" % (Ci, Cin))
     if (PW_FWD and KH == 1 and KW == 1 and stride == 1 and padding == 0 and groups == 1 and not upsample2
             and zero_stuff_out is None and pre_scale is None and not pre_relu and stats is None and bn_bwd is None
-            and precision == 0 and packed is None and act in ACT and B * Hs * Ws >= PW_MIN_PIXELS
+            and precision in (None, 0) and packed is None and act in ACT and B * Hs * Ws >= PW_MIN_PIXELS
             and xs % 4 == 0 and x.data_ptr() % 16 == 0 and _lib.lib().bts_conv_pw_fwd_eligible(Cin, Co)):
         # narrow 1x1 layers of the reduction heads (forward and dgrad): HBM-bound CUDA-core kernel (csrc/pointwise.cu)
         if out is None:
@@ -230,6 +268,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         _lib.check(rc, "bts_conv_pw_fwd")
         _lib.count()
         return out
+    precision = _engine_precision(precision)
     if packed is None:
         packed = pack_weights(weight, transpose_flip, groups)
     if zero_stuff_out is not None:
@@ -292,8 +331,8 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
     return out
 
 
-def wgrad_grouped_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=1, precision=0):
-    """dW of a grouped (block-diagonal) 3x3 conv: weight (width, cpg, KH, KW)"""
+def wgrad_grouped_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=1, precision=None):
+    """dW of a grouped (block-diagonal) 3x3 conv: weight (width, cpg, KH, KW).  precision: as conv2d_tc"""
     _need_cuda(x, gy)
     x, xs = _nhwc_view(x)
     gy, gs = _nhwc_view(gy)
@@ -311,7 +350,7 @@ def wgrad_grouped_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, d
         rc = _traced("wgrad", "%dx%dx%d %d->%d k%d d%d s%d g%d" % (B, Hs, Ws, width, width, KH, dilation, stride, width // cpg),
                      lambda: L.bts_conv_wgrad_grouped(_ptr(x), xs, B, Hs, Ws, width, cpg, KH, KW, stride, padding, dilation,
                                                       _ptr(gy), gs, _ptr(ws), split.value, _ptr(gw), s[0], s[1], s[2], s[3],
-                                                      int(precision), _stream()),
+                                                      _engine_precision(precision), _stream()),
                      2.0 * B * gy.shape[2] * gy.shape[3] * width * cpg * KH * KW)
     _lib.check(rc, "bts_conv_wgrad_grouped")
     _lib.count(2)
@@ -319,8 +358,8 @@ def wgrad_grouped_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, d
 
 
 def wgrad_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=1, pre_scale=None, pre_shift=None,
-             pre_relu=False, upsample2=False, precision=0):
-    """dW (shaped/strided like the weight parameter) on the wgmma engine."""
+             pre_relu=False, upsample2=False, precision=None):
+    """dW (shaped/strided like the weight parameter) on the wgmma engine.  precision: as conv2d_tc"""
     _need_cuda(x, gy)
     x, xs = _nhwc_view(x)
     gy, gs = _nhwc_view(gy)
@@ -328,7 +367,7 @@ def wgrad_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=
     Cout, _, KH, KW = weight_shape
     L = _lib.lib()
     if (PW_WGRAD and KH == 1 and KW == 1 and stride == 1 and padding == 0 and pre_scale is None and not pre_relu
-            and not upsample2 and precision == 0 and B * Hs * Ws >= PW_MIN_PIXELS and L.bts_conv_pw_wgrad_eligible(Cin, Cout)):
+            and not upsample2 and precision in (None, 0) and B * Hs * Ws >= PW_MIN_PIXELS and L.bts_conv_pw_wgrad_eligible(Cin, Cout)):
         # narrow 1x1 layers of the reduction heads: HBM-bound CUDA-core kernel (csrc/pointwise.cu)
         ws = torch.empty(L.bts_conv_pw_wgrad_workspace_floats(Cin, Cout), device=x.device, dtype=torch.float32)
         gw = torch.empty_strided(tuple(weight_shape), tuple(weight_strides), device=x.device, dtype=torch.float32)
@@ -340,6 +379,7 @@ def wgrad_tc(x, gy, weight_shape, weight_strides, stride=1, padding=0, dilation=
         _lib.check(rc, "bts_conv_pw_wgrad")
         _lib.count(2)
         return gw
+    precision = _engine_precision(precision)
     split = ctypes.c_int(0)
     wsf = ctypes.c_longlong(0)
     _lib.check(L.bts_conv_wgrad_plan(B, gy.shape[2], gy.shape[3], Cin, Cout, KH, KW, stride, ctypes.byref(split), ctypes.byref(wsf)),

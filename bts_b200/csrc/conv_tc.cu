@@ -18,7 +18,9 @@
 // A_lo*B_hi + A_hi*B_lo + A_hi*B_hi  with tf32 wgmma into fp32 register accumulators (error ~2^-21 per product:
 // fp32-grade, SURVEY Appendix F); every k-block's tensor-core sum is added into the tile sum with round-to-nearest fp32
 // adds.  The weights are split once, when they are packed; the activations are split by the consumers in registers.
-// Single-pass TF32 is available as an explicitly labelled fast mode (precision=1) and is NOT used for parity.
+// Single-pass TF32 (precision=1, opt-in) runs conv_tf32_kernel, the same body compiled for one product: A and B_hi
+// only, A_hi*B_hi per k8 step.  Its stage is A + B_hi (the producers' bulk copy fetches only the hi half of each packed
+// k-block), so more stages fit; the k-block order, the tile sum and the epilogue are those of conv_tc_kernel.
 //
 // Persistent kernel: grid = min(#tiles, #SMs); every CTA walks tiles blockIdx.x, +gridDim.x, ... with the smem stage
 // ring and all warp roles running continuously across tile boundaries (the producers fill the stages of tile t+1 while
@@ -80,7 +82,6 @@ struct ConvParams {
     long long os;
     int Hout, Wout;
     int act;                 // 0 none, 1 ELU, 2 sigmoid
-    int precision;           // 0: 3xTF32 (parity), 1: 1xTF32 (fast, labelled)
     int vec_ok;              // 16-byte aligned rows -> float4 loads
     long long M;             // B*Hout*Wout
     int m_tiles, total_tiles;
@@ -94,7 +95,7 @@ struct ConvParams {
     const float *bnb_x; long long bnb_xs;
     const float *bnb_st;             // [4][Cout]: scale, shift, mean, invstd
     int bnb_relu;
-    int stages, stage_bytes; // smem ring: as many (A + B hi/lo) stages as fit
+    int stages, stage_bytes; // smem ring: as many (A + B hi/lo, single pass: A + B hi) stages as fit
     tc::FastDiv fd_wout, fd_hout, fd_ntiles;
 };
 
@@ -198,6 +199,7 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackDesc 
 // ------------------------------------------------------------------------------------------- main kernel
 // dynamic smem, 1024-byte aligned base:
 //   [S stages][A 16K | B_hi n_tile*128 | B_lo n_tile*128]   S = as many stages as fit (2..MAX_STAGES)
+//   (single pass: [A 16K | B_hi n_tile*128] per stage)
 //   [pre-op scale[KC*32], shift[KC*32]]  (PRE >= 2 only)   [mbarriers]   [epilogue statistics partials]
 constexpr int MAX_STAGES = 6;
 constexpr int SMEM_LIMIT = 232448;          // 227 KB opt-in maximum per CTA
@@ -211,8 +213,9 @@ constexpr int STAT_SETS = CONSUMER_THREADS / 32;
 //
 // Index arithmetic: every k-block -> (tile, tap, channel chunk, stage, phase) mapping is carried in incrementally updated
 // counters, and the per-tile pixel decode uses multiply-shift division by host-precomputed constants (FastDiv).
-template <int PRE, int UP, bool VEC>
-__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParams p) {
+// SINGLE: single-pass TF32 (conv_tf32_kernel) instead of 3xTF32 (conv_tc_kernel).
+template <int PRE, int UP, bool VEC, bool SINGLE>
+__device__ __forceinline__ void conv_body(const ConvParams &p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16-byte aligned: round up to 1024 (SWIZZLE_128B atoms)
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -268,7 +271,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
         const int grp = pt / PRODUCER_THREADS;     // producer group: global k-blocks gk == grp (mod 2)
         const int t = pt % PRODUCER_THREADS;
         const bool issuer = t == 0;
-        const uint32_t wbytes = 2u * (uint32_t)n_tile * 128u;
+        const uint32_t wstride = 2u * (uint32_t)n_tile * 128u;           // one packed k-block: [hi | lo] rows
+        const uint32_t wbytes = SINGLE ? wstride / 2u : wstride;          // single pass: the hi half only
         const uint8_t *wsrc = reinterpret_cast<const uint8_t *>(p.wpack);
         const int chunk = t & 7;                   // 16-byte chunk of the 128-byte row
         const int r0 = t >> 3;                     // rows r0 + 16*i, i = 0..7  (row & 7 == r0 & 7 for all of them)
@@ -378,7 +382,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
             mbar_wait(empty(s_s), s_ph ^ 1);
             if (issuer) {
                 mbar_arrive_expect_tx(bar_full, wbytes);
-                bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + (size_t)w * wbytes, wbytes, bar_full);
+                bulk_copy_g2s(stage + A_TILE_BYTES, wsrc + (size_t)w * wstride, wbytes, bar_full);
             }
             uint32_t mk = 0;
 #pragma unroll
@@ -437,10 +441,10 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
         // The tensor cores accumulate one k-block (4 k8 steps x 3 products) into `acc`; it is then added into the fp32
         // tile sum `tot` with round-to-nearest adds, which keeps the accumulation error of long-K layers at the level of a
         // plain fp32 sum.  The stage is handed back to the producers as soon as its wgmma group has completed.
+        // Single pass: A rounded like hi above, one product A_hi*B_hi per k8 step, the same k-block sums.
         const int wg = warp >> 2;
         const int row = wg * 64 + (warp & 3) * 16 + (lane >> 2);     // rows row and row + 8 of the tile
         const bool ovec = ((p.os & 1) == 0) && ((((uintptr_t)p.out) & 7) == 0);
-        const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             constexpr int R = N / 2;
@@ -463,23 +467,38 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
                 for (int i = 0; i < R; ++i) tot[i] = 0.f;
                 for (int kb = 0; kb < KB; ++kb) {
                     mbar_wait_no_trap(full(s), ph);
-                    uint32_t hi[BLOCK_K / 8][4], lo[BLOCK_K / 8][4];
+                    if constexpr (SINGLE) {
+                        uint32_t hi[BLOCK_K / 8][4];
 #pragma unroll
-                    for (int k = 0; k < BLOCK_K / 8; ++k) {
+                        for (int k = 0; k < BLOCK_K / 8; ++k) {
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {                      // j: row + 8 (j & 1), column + 4 (j >> 1)
-                            const uint32_t x = ld_shared_u32((aF ^ (uint32_t)(32 * k + 16 * (j >> 1))) + 1024u * (j & 1));
-                            float h, l;
-                            split_tf32(__uint_as_float(x), h, l);
-                            hi[k][j] = __float_as_uint(h);
-                            lo[k][j] = __float_as_uint(l);
+                            for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
+                                const uint32_t x = ld_shared_u32((aF ^ (uint32_t)(32 * k + 16 * (j >> 1))) + 1024u * (j & 1));
+                                hi[k][j] = __float_as_uint(round_tf32(__uint_as_float(x)));
+                            }
                         }
-                    }
-                    wgmma_fence();
-                    if (single) {
+                        wgmma_fence();
 #pragma unroll
                         for (int k = 0; k < BLOCK_K / 8; ++k) Wgmma<N>::mma_rs(acc, hi[k], d + 2 * k, k != 0);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_operands(acc);
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 8; ++k) wgmma_fence_operands(hi[k]);
                     } else {
+                        uint32_t hi[BLOCK_K / 8][4], lo[BLOCK_K / 8][4];
+#pragma unroll
+                        for (int k = 0; k < BLOCK_K / 8; ++k) {
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
+                                const uint32_t x = ld_shared_u32((aF ^ (uint32_t)(32 * k + 16 * (j >> 1))) + 1024u * (j & 1));
+                                float h, l;
+                                split_tf32(__uint_as_float(x), h, l);
+                                hi[k][j] = __float_as_uint(h);
+                                lo[k][j] = __float_as_uint(l);
+                            }
+                        }
+                        wgmma_fence();
 #pragma unroll
                         for (int k = 0; k < BLOCK_K / 8; ++k) {
                             const uint64_t dbh = d + 2 * k, dbl = dbh + oBlo;
@@ -487,14 +506,14 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
                             Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
                             Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
                         }
-                    }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    wgmma_fence_operands(acc);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_operands(acc);
 #pragma unroll
-                    for (int k = 0; k < BLOCK_K / 8; ++k) {
-                        wgmma_fence_operands(hi[k]);
-                        wgmma_fence_operands(lo[k]);
+                        for (int k = 0; k < BLOCK_K / 8; ++k) {
+                            wgmma_fence_operands(hi[k]);
+                            wgmma_fence_operands(lo[k]);
+                        }
                     }
                     __syncwarp();
                     if (lane == 0) mbar_arrive(empty(s));
@@ -631,6 +650,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParam
     }
 }
 
+template <int PRE, int UP, bool VEC>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const ConvParams p) {
+    conv_body<PRE, UP, VEC, false>(p);
+}
+
+template <int PRE, int UP, bool VEC>
+__global__ void __launch_bounds__(NUM_THREADS, 1) conv_tf32_kernel(const ConvParams p) {
+    conv_body<PRE, UP, VEC, true>(p);
+}
 
 }  // namespace
 
@@ -752,7 +780,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.n_tile = kwin ? bts_conv_group_n_tile(kwin) : bts_conv_n_tile(Cout);
     p.n_tiles = (Cout + p.n_tile - 1) / p.n_tile;
     p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu ? 1 : 0;
-    p.out = out; p.os = out_pixel_stride; p.act = act; p.precision = precision;
+    p.out = out; p.os = out_pixel_stride; p.act = act;
     p.stat_sum = stat_sum; p.stat_sumsq = stat_sumsq;
     if ((stat_sum == nullptr) != (stat_sumsq == nullptr)) return BTS_EINVAL;
     p.bnb_x = nullptr; p.bnb_xs = 0; p.bnb_st = nullptr; p.bnb_relu = 0;
@@ -785,8 +813,8 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     p.fd_ntiles = make_fastdiv((uint32_t)p.n_tiles);
     const int pre = (pre_scale ? 2 : 0) | (p.pre_relu ? 1 : 0);
-    // shared-memory plan: stage = A (16 KB) + B hi/lo (2 x n_tile x 128 B); as many stages as fit
-    p.stage_bytes = A_TILE_BYTES + 2 * p.n_tile * 128;
+    // shared-memory plan: stage = A (16 KB) + B hi/lo (2 x n_tile x 128 B), single pass A + B hi; as many stages as fit
+    p.stage_bytes = A_TILE_BYTES + (precision ? 1 : 2) * p.n_tile * 128;
     const int pre_bytes = pre >= 2 ? p.KC * 32 * 8 : 0;
     const int stat_bytes = stat_sum ? STAT_SETS * 2 * p.n_tile * 8 : 0;
     p.stages = (SMEM_LIMIT - 1024 - BAR_BYTES - pre_bytes - stat_bytes) / p.stage_bytes;
@@ -797,30 +825,36 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     dim3 grid((unsigned)(p.total_tiles < sms ? p.total_tiles : sms));
     const bool vec = p.vec_ok;      // aligned base + pixel stride % 4 == 0 (a channel tail is masked in-kernel)
     cudaError_t err = cudaSuccess;
-#define BTS_LAUNCH(PRE, UP, VEC)                                                                                   \
+#define BTS_LAUNCH(KERNEL, PRE, UP, VEC)                                                                           \
     do {                                                                                                           \
         static bool attr_set_[BTS_MAX_DEVICES] = {};                                                               \
         bool &attr_set = attr_set_[bts_cur_device()];                                                              \
         if (!attr_set) {                                                                                           \
-            err = cudaFuncSetAttribute(conv_tc_kernel<PRE, UP, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+            err = cudaFuncSetAttribute(KERNEL<PRE, UP, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,          \
                                        SMEM_LIMIT);                                                                \
             if (err != cudaSuccess) return (int)err;                                                               \
             attr_set = true;                                                                                       \
         }                                                                                                          \
-        conv_tc_kernel<PRE, UP, VEC><<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(p);                        \
+        KERNEL<PRE, UP, VEC><<<grid, NUM_THREADS, smem, (cudaStream_t)stream>>>(p);                                \
     } while (0)
-#define BTS_DISPATCH_UV(PRE)                                                                                       \
+#define BTS_DISPATCH_UV(KERNEL, PRE)                                                                               \
     do {                                                                                                           \
-        if (p.up == 2) { if (vec) BTS_LAUNCH(PRE, 2, true); else BTS_LAUNCH(PRE, 2, false); }                      \
-        else if (p.up) { if (vec) BTS_LAUNCH(PRE, 1, true); else BTS_LAUNCH(PRE, 1, false); }                      \
-        else { if (vec) BTS_LAUNCH(PRE, 0, true); else BTS_LAUNCH(PRE, 0, false); }                                \
+        if (p.up == 2) { if (vec) BTS_LAUNCH(KERNEL, PRE, 2, true); else BTS_LAUNCH(KERNEL, PRE, 2, false); }      \
+        else if (p.up) { if (vec) BTS_LAUNCH(KERNEL, PRE, 1, true); else BTS_LAUNCH(KERNEL, PRE, 1, false); }      \
+        else { if (vec) BTS_LAUNCH(KERNEL, PRE, 0, true); else BTS_LAUNCH(KERNEL, PRE, 0, false); }                \
     } while (0)
-    switch (pre) {
-        case 0: BTS_DISPATCH_UV(0); break;
-        case 1: BTS_DISPATCH_UV(1); break;
-        case 2: BTS_DISPATCH_UV(2); break;
-        default: BTS_DISPATCH_UV(3); break;
-    }
+#define BTS_DISPATCH(KERNEL)                                                                                       \
+    do {                                                                                                           \
+        switch (pre) {                                                                                             \
+            case 0: BTS_DISPATCH_UV(KERNEL, 0); break;                                                             \
+            case 1: BTS_DISPATCH_UV(KERNEL, 1); break;                                                             \
+            case 2: BTS_DISPATCH_UV(KERNEL, 2); break;                                                             \
+            default: BTS_DISPATCH_UV(KERNEL, 3); break;                                                            \
+        }                                                                                                          \
+    } while (0)
+    if (precision) BTS_DISPATCH(conv_tf32_kernel);
+    else BTS_DISPATCH(conv_tc_kernel);
+#undef BTS_DISPATCH
 #undef BTS_DISPATCH_UV
 #undef BTS_LAUNCH
     BTS_LAUNCH_CHECK();

@@ -110,11 +110,16 @@ __device__ __forceinline__ float rna_tf32(float x) {
     return __uint_as_float(r);
 }
 
-// 3xTF32 operand split x = hi + lo: hi = x rounded to tf32 (round-half-away on the 13 dropped mantissa bits, two integer
-// ops), lo = x - hi, exact in fp32.  The tensor cores read the top 19 bits of each word, so hi*hi + hi*lo + lo*hi leaves
-// about 2^-21 relative per product.
+// x rounded to tf32: round-half-away on the 13 dropped mantissa bits, two integer ops.  The hi half of split_tf32, and
+// the operand of the single-pass TF32 kernels, which therefore compute exactly the A_hi*B_hi product of the 3xTF32 ones.
+__device__ __forceinline__ float round_tf32(float x) {
+    return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+}
+
+// 3xTF32 operand split x = hi + lo: hi = round_tf32(x), lo = x - hi, exact in fp32.  The tensor cores read the top 19
+// bits of each word, so hi*hi + hi*lo + lo*hi leaves about 2^-21 relative per product.
 __device__ __forceinline__ void split_tf32(float x, float &hi, float &lo) {
-    hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
+    hi = round_tf32(x);
     lo = x - hi;
 }
 

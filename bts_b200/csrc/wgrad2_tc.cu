@@ -15,6 +15,8 @@
 //   B = dY: K-major (pixels contiguous per column) hi/lo tiles of 8 x 16-byte core matrices, transposed by the producers.
 // Deterministic split-K partial layout as wgrad_tc.cu; split-K ranges are whole multiples of 16 pixels.
 // 512 threads (16 warps, 128 registers per thread): 2 consumer warpgroups + 2 producer warpgroups.
+// Single-pass TF32 (precision=1, opt-in) runs wgrad2_tf32_kernel, the same body compiled for one product: one dY tile
+// (hi) per stage and A_hi*B_hi per k8 step.
 //
 // Operand staging: the shifted dY windows of a k-block overlap -- they are KH row segments of 32 + (KW-1)*dil consecutive
 // output pixels.  With TMA = true one producer lane copies the raw fp32 segments (and the raw x tile unless it is read
@@ -59,14 +61,14 @@ struct W2Params {
     float *part;             // [splitK][taps][Cin][Cout]
     int splitK, px_per_split;
     int Mq;                  // B*Hin*Win input pixels
-    int stages, stage_bytes, b_half, precision;   // stage = [x X_BYTES | dY hi b_half | dY lo b_half]
+    int stages, stage_bytes, b_half;   // stage = [x X_BYTES | dY hi b_half | dY lo b_half] (single pass: no lo)
     // TMA landing ring (TMA = true): slot = [raw x tile (unless up) | KH segments of segw pixels x cg channels]
     int ring, slot_bytes, seg_bytes, segw, tox_max, slot_tx;
 };
 
-template <int PRE, bool UP, bool VEC, bool TMA>
-__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Params p, const __grid_constant__ CUtensorMap tmx,
-                                                                   const __grid_constant__ CUtensorMap tmd) {
+// SINGLE: single-pass TF32 (wgrad2_tf32_kernel) instead of 3xTF32 (wgrad2_tc_kernel)
+template <int PRE, bool UP, bool VEC, bool TMA, bool SINGLE>
+__device__ __forceinline__ void wgrad2_body(const W2Params &p, const CUtensorMap &tmx, const CUtensorMap &tmd) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
@@ -131,7 +133,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
         const int q = lane & 3;
         const int c = (warp & 3) * 16 + (lane >> 2);
         const uint32_t aF = (uint32_t)q * X_ROW_BYTES + ((uint32_t)((c >> 2) ^ (2 * q)) << 4) + (uint32_t)(c & 3) * 4u;
-        const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             float acc[N > 0 ? N / 2 : 1];
@@ -143,40 +144,60 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
                 mbar_wait(full(s), ph);
                 if constexpr (N > 0) {
                     const uint32_t st = base + (uint32_t)s * stage_bytes;
-                    uint32_t hi[KP / 8][4], lo[KP / 8][4];
+                    if constexpr (SINGLE) {
+                        uint32_t hi[KP / 8][4];
 #pragma unroll
-                    for (int k = 0; k < KP / 8; ++k) {
+                        for (int k = 0; k < KP / 8; ++k) {
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
-                            const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
-                            float h, l;
-                            split_tf32(__uint_as_float(x), h, l);
-                            hi[k][j] = __float_as_uint(h);
-                            lo[k][j] = __float_as_uint(l);
+                            for (int j = 0; j < 4; ++j) {              // j: row + 8 (j & 1), column + 4 (j >> 1)
+                                const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                                hi[k][j] = __float_as_uint(round_tf32(__uint_as_float(x)));
+                            }
                         }
-                    }
-                    const uint32_t b_hi = st + X_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO, b_lo = b_hi + (uint32_t)p.b_half;
-                    wgmma_fence();
+                        const uint32_t b_hi = st + X_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO;
+                        wgmma_fence();
 #pragma unroll
-                    for (int k = 0; k < KP / 8; ++k) {
-                        const uint32_t ko = (uint32_t)k * 256u;
-                        const uint64_t dbh = make_desc_core(b_hi + ko, 128, CORE_SBO), dbl = make_desc_core(b_lo + ko, 128, CORE_SBO);
-                        const uint32_t accumulate = (it | k) != 0;
-                        if (single) {
-                            Wgmma<N>::mma_rs(acc, hi[k], dbh, accumulate);
-                        } else {
+                        for (int k = 0; k < KP / 8; ++k) {
+                            const uint64_t dbh = make_desc_core(b_hi + (uint32_t)k * 256u, 128, CORE_SBO);
+                            Wgmma<N>::mma_rs(acc, hi[k], dbh, (it | k) != 0);
+                        }
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_operands(acc);
+#pragma unroll
+                        for (int k = 0; k < KP / 8; ++k) wgmma_fence_operands(hi[k]);
+                    } else {
+                        uint32_t hi[KP / 8][4], lo[KP / 8][4];
+#pragma unroll
+                        for (int k = 0; k < KP / 8; ++k) {
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {              // j: row + 8 (j & 1), column + 4 (j >> 1)
+                                const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                                float h, l;
+                                split_tf32(__uint_as_float(x), h, l);
+                                hi[k][j] = __float_as_uint(h);
+                                lo[k][j] = __float_as_uint(l);
+                            }
+                        }
+                        const uint32_t b_hi = st + X_BYTES + (uint32_t)(n0 >> 3) * CORE_SBO, b_lo = b_hi + (uint32_t)p.b_half;
+                        wgmma_fence();
+#pragma unroll
+                        for (int k = 0; k < KP / 8; ++k) {
+                            const uint32_t ko = (uint32_t)k * 256u;
+                            const uint64_t dbh = make_desc_core(b_hi + ko, 128, CORE_SBO), dbl = make_desc_core(b_lo + ko, 128, CORE_SBO);
+                            const uint32_t accumulate = (it | k) != 0;
                             Wgmma<N>::mma_rs(acc, lo[k], dbh, accumulate);
                             Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
                             Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
                         }
-                    }
-                    wgmma_commit();
-                    wgmma_wait<0>();
-                    wgmma_fence_operands(acc);
+                        wgmma_commit();
+                        wgmma_wait<0>();
+                        wgmma_fence_operands(acc);
 #pragma unroll
-                    for (int k = 0; k < KP / 8; ++k) {
-                        wgmma_fence_operands(hi[k]);
-                        wgmma_fence_operands(lo[k]);
+                        for (int k = 0; k < KP / 8; ++k) {
+                            wgmma_fence_operands(hi[k]);
+                            wgmma_fence_operands(lo[k]);
+                        }
                     }
                 }
                 mbar_arrive(empty(s));
@@ -238,8 +259,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
         const int cbx = ci_tile * BLOCK_CI + ul * 4;                  // first x channel of this thread's first unit
         const float *__restrict__ xg = p.x;
         const float *__restrict__ dg = p.dy;
+        // The pre-op's scale / shift stay in 16 registers, except on the scalar-load path (VEC = false), which holds four
+        // times the loads in flight: it reads them from shared memory at each use and so stays within 128 registers
+        // without spills (the same values: the same results).
+        constexpr bool AFF_REGS = AFF && VEC;
         float sc[2][4], sh[2][4];
-        if (AFF) {
+        if (AFF_REGS) {
 #pragma unroll
             for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -378,7 +403,8 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
 #pragma unroll
                 for (int e = 0; e < 4; ++e) {
                     float a = va[h].v[e];
-                    if (AFF) a = fmaf(a, sc[h][e], sh[h][e]);
+                    if (AFF_REGS) a = fmaf(a, sc[h][e], sh[h][e]);
+                    else if (AFF) a = fmaf(a, s_scale[h * 32 + ul * 4 + e], s_shift[h * 32 + ul * 4 + e]);
                     if (RELU) a = fmaxf(a, 0.f);
                     va[h].v[e] = okx ? a : 0.f;        // pixels past this CTA's range (zero padding after the pre-op)
                 }
@@ -391,13 +417,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
 #pragma unroll
             for (int ch = 0; ch < MAX_CHUNKS; ++ch) {
                 if (!blive[ch]) continue;
-                float hi[4], lo[4];
+                if constexpr (SINGLE) {
 #pragma unroll
-                for (int e = 0; e < 4; ++e) split_tf32(vb[ch].v[e], hi[e], lo[e]);
+                    for (int e = 0; e < 4; ++e) st_shared_f32(b_hi + boff[ch] + 16u * e, round_tf32(vb[ch].v[e]));
+                } else {
+                    float hi[4], lo[4];
 #pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    st_shared_f32(b_hi + boff[ch] + 16u * e, hi[e]);
-                    st_shared_f32(b_lo + boff[ch] + 16u * e, lo[e]);
+                    for (int e = 0; e < 4; ++e) split_tf32(vb[ch].v[e], hi[e], lo[e]);
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        st_shared_f32(b_hi + boff[ch] + 16u * e, hi[e]);
+                        st_shared_f32(b_lo + boff[ch] + 16u * e, lo[e]);
+                    }
                 }
             }
             fence_proxy_async();                       // generic-proxy dY writes -> visible to wgmma (async proxy)
@@ -465,6 +496,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Param
             }
         }
     }
+}
+
+template <int PRE, bool UP, bool VEC, bool TMA>
+__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tc_kernel(const W2Params p, const __grid_constant__ CUtensorMap tmx,
+                                                                   const __grid_constant__ CUtensorMap tmd) {
+    wgrad2_body<PRE, UP, VEC, TMA, false>(p, tmx, tmd);
+}
+
+template <int PRE, bool UP, bool VEC, bool TMA>
+__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad2_tf32_kernel(const W2Params p, const __grid_constant__ CUtensorMap tmx,
+                                                                     const __grid_constant__ CUtensorMap tmd) {
+    wgrad2_body<PRE, UP, VEC, TMA, true>(p, tmx, tmd);
 }
 
 }  // namespace
@@ -576,11 +619,10 @@ int bts_wgrad2_launch(const float *x, long long xs, int B, int Hs, int Ws, int u
     const int blocks = (int)((Mq + SPLIT_PX - 1) / SPLIT_PX);
     p.px_per_split = (blocks + splitK - 1) / splitK * SPLIT_PX;
     p.b_half = taps * p.cg / 8 * (int)CORE_SBO;
-    p.stage_bytes = (X_BYTES + 2 * p.b_half + 127) / 128 * 128;     // TMA ring slots that follow stay 128-byte aligned
+    p.stage_bytes = (X_BYTES + (precision ? 1 : 2) * p.b_half + 127) / 128 * 128;   // ring slots stay 128-byte aligned
     p.stages = SMEM_BUDGET / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     if (p.stages < 2) return BTS_EINVAL;
-    p.precision = precision;
     const int pre = (pre_scale ? 2 : 0) | (pre_relu ? 1 : 0);
     const bool vec = bts_aligned16(x) && (xs % 4 == 0) && bts_aligned16(dy) && (dys % 4 == 0);
     // ---- landing ring (TMA): 'same' convolutions with <= 3 kernel rows; 3 operand stages if >= 3 ring slots still fit, else 2
@@ -617,29 +659,35 @@ int bts_wgrad2_launch(const float *x, long long xs, int B, int Hs, int Ws, int u
     const int smem = p.stages * p.stage_bytes + p.ring * p.slot_bytes + 2 * BLOCK_CI * 4 + 256 + 1024;
     dim3 grid((Cin + BLOCK_CI - 1) / BLOCK_CI, (Cout + p.cg - 1) / p.cg, splitK);
     cudaError_t err = cudaSuccess;
-#define BTS_LAUNCH(PRE, UP, VEC, TMA)                                                                                 \
+#define BTS_LAUNCH(KERNEL, PRE, UP, VEC, TMA)                                                                         \
     do {                                                                                                              \
         static int attr_smem_[BTS_MAX_DEVICES] = {}; int &attr_smem = attr_smem_[bts_cur_device()];                   \
         if (attr_smem < smem) {                                                                                       \
-            err = cudaFuncSetAttribute(wgrad2_tc_kernel<PRE, UP, VEC, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, \
+            err = cudaFuncSetAttribute(KERNEL<PRE, UP, VEC, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize,        \
                                        SMEM_BUDGET + 2 * BLOCK_CI * 4 + 256 + 1024);                                  \
             if (err != cudaSuccess) return (int)err;                                                                  \
             attr_smem = SMEM_BUDGET + 2 * BLOCK_CI * 4 + 256 + 1024;                                                  \
         }                                                                                                             \
-        wgrad2_tc_kernel<PRE, UP, VEC, TMA><<<grid, NUM_THREADS, smem, st>>>(p, tmx, tmd);                            \
+        KERNEL<PRE, UP, VEC, TMA><<<grid, NUM_THREADS, smem, st>>>(p, tmx, tmd);                                      \
     } while (0)
-#define BTS_DISPATCH_UV(PRE)                                                                     \
-    do {                                                                                         \
-        if (tma) { if (p.up) BTS_LAUNCH(PRE, true, true, true); else BTS_LAUNCH(PRE, false, true, true); } \
-        else if (p.up) { if (vec) BTS_LAUNCH(PRE, true, true, false); else BTS_LAUNCH(PRE, true, false, false); }   \
-        else { if (vec) BTS_LAUNCH(PRE, false, true, false); else BTS_LAUNCH(PRE, false, false, false); }      \
+#define BTS_DISPATCH_UV(KERNEL, PRE)                                                                                  \
+    do {                                                                                                              \
+        if (tma) { if (p.up) BTS_LAUNCH(KERNEL, PRE, true, true, true); else BTS_LAUNCH(KERNEL, PRE, false, true, true); } \
+        else if (p.up) { if (vec) BTS_LAUNCH(KERNEL, PRE, true, true, false); else BTS_LAUNCH(KERNEL, PRE, true, false, false); } \
+        else { if (vec) BTS_LAUNCH(KERNEL, PRE, false, true, false); else BTS_LAUNCH(KERNEL, PRE, false, false, false); } \
     } while (0)
-    switch (pre) {
-        case 0: BTS_DISPATCH_UV(0); break;
-        case 1: BTS_DISPATCH_UV(1); break;
-        case 2: BTS_DISPATCH_UV(2); break;
-        default: BTS_DISPATCH_UV(3); break;
-    }
+#define BTS_DISPATCH(KERNEL)                                                                                          \
+    do {                                                                                                              \
+        switch (pre) {                                                                                                \
+            case 0: BTS_DISPATCH_UV(KERNEL, 0); break;                                                                \
+            case 1: BTS_DISPATCH_UV(KERNEL, 1); break;                                                                \
+            case 2: BTS_DISPATCH_UV(KERNEL, 2); break;                                                                \
+            default: BTS_DISPATCH_UV(KERNEL, 3); break;                                                               \
+        }                                                                                                             \
+    } while (0)
+    if (precision) BTS_DISPATCH(wgrad2_tf32_kernel);
+    else BTS_DISPATCH(wgrad2_tc_kernel);
+#undef BTS_DISPATCH
 #undef BTS_DISPATCH_UV
 #undef BTS_LAUNCH
     BTS_LAUNCH_CHECK();

@@ -12,6 +12,8 @@
 // and writes a partial; a second, deterministic kernel sums the splitK partials into the (Cout,Cin,KH,KW)-strided gradient.
 // 512 threads (16 warps, 128 registers per thread): 2 consumer warpgroups + 2 producer warpgroups (x tile / dY tile),
 // 2-6 operand stages.
+// Single-pass TF32 (precision=1, opt-in) runs wgrad_tf32_kernel, the same body compiled for one product: the dY producers
+// write only the hi tile, a stage is x + dY hi, and the consumers issue A_hi*B_hi per k8 step (A rounded as hi is).
 #include <cstdlib>
 #include <type_traits>
 
@@ -45,15 +47,16 @@ struct WgradParams {
     float *part;             // [splitK][taps][Cin][Cout]   (grouped: [splitK][taps][Cin][kwin])
     int splitK, kb_per_split, KBp;
     int M;
-    int x_vec, dy_vec, precision;
-    int stages, stage_bytes;     // operand ring: [x X_BYTES | dY hi b_bytes | dY lo b_bytes] per stage
+    int x_vec, dy_vec;
+    int stages, stage_bytes;     // operand ring: [x X_BYTES | dY hi b_bytes | dY lo b_bytes] per stage (single pass: no lo)
     int b_bytes;
     FastDiv fd_wout, fd_hout;
 };
 
 
-template <int PRE, bool UP, bool VEC>
-__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradParams p) {
+// SINGLE: single-pass TF32 (wgrad_tf32_kernel) instead of 3xTF32 (wgrad_tc_kernel)
+template <int PRE, bool UP, bool VEC, bool SINGLE>
+__device__ __forceinline__ void wgrad_body(const WgradParams &p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t *sm = smem_raw + (base - smem_u32(smem_raw));
@@ -110,7 +113,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
         const int q = lane & 3;
         const int c = wg * 64 + (warp & 3) * 16 + (lane >> 2);
         const uint32_t aF = (uint32_t)q * X_ROW_BYTES + ((uint32_t)((c >> 2) ^ (2 * q)) << 4) + (uint32_t)(c & 3) * 4u;
-        const bool single = p.precision != 0;
         auto consume = [&](auto NT) {
             constexpr int N = decltype(NT)::value;
             float acc[N / 2];
@@ -121,39 +123,58 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             for (int it = 0; it < nkb; ++it) {
                 mbar_wait(full(s), ph);
                 const uint32_t st = base + (uint32_t)s * stage_bytes;
-                uint32_t hi[BLOCK_KP / 8][4], lo[BLOCK_KP / 8][4];
+                if constexpr (SINGLE) {
+                    uint32_t hi[BLOCK_KP / 8][4];
 #pragma unroll
-                for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) {
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {                      // j: row + 8 (j & 1), column + 4 (j >> 1)
-                        const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
-                        float h, l;
-                        split_tf32(__uint_as_float(x), h, l);
-                        hi[k][j] = __float_as_uint(h);
-                        lo[k][j] = __float_as_uint(l);
+                        for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
+                            const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                            hi[k][j] = __float_as_uint(round_tf32(__uint_as_float(x)));
+                        }
                     }
-                }
-                wgmma_fence();
+                    wgmma_fence();
 #pragma unroll
-                for (int k = 0; k < BLOCK_KP / 8; ++k) {
-                    const uint32_t ko = (uint32_t)k * 256u;
-                    const uint64_t dbh = make_desc_core(st + b_off + ko, 128, CORE_SBO), dbl = make_desc_core(st + bl_off + ko, 128, CORE_SBO);
-                    const uint32_t accumulate = (it | k) != 0;
-                    if (single) {
-                        Wgmma<N>::mma_rs(acc, hi[k], dbh, accumulate);
-                    } else {
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                        const uint64_t dbh = make_desc_core(st + b_off + (uint32_t)k * 256u, 128, CORE_SBO);
+                        Wgmma<N>::mma_rs(acc, hi[k], dbh, (it | k) != 0);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_operands(acc);
+#pragma unroll
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) wgmma_fence_operands(hi[k]);
+                } else {
+                    uint32_t hi[BLOCK_KP / 8][4], lo[BLOCK_KP / 8][4];
+#pragma unroll
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) {
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {                  // j: row + 8 (j & 1), column + 4 (j >> 1)
+                            const uint32_t x = ld_shared_u32(st + (aF ^ (32u * (j & 1))) + (uint32_t)(8 * k + 4 * (j >> 1)) * X_ROW_BYTES);
+                            float h, l;
+                            split_tf32(__uint_as_float(x), h, l);
+                            hi[k][j] = __float_as_uint(h);
+                            lo[k][j] = __float_as_uint(l);
+                        }
+                    }
+                    wgmma_fence();
+#pragma unroll
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                        const uint32_t ko = (uint32_t)k * 256u;
+                        const uint64_t dbh = make_desc_core(st + b_off + ko, 128, CORE_SBO), dbl = make_desc_core(st + bl_off + ko, 128, CORE_SBO);
+                        const uint32_t accumulate = (it | k) != 0;
                         Wgmma<N>::mma_rs(acc, lo[k], dbh, accumulate);
                         Wgmma<N>::mma_rs(acc, hi[k], dbl, 1);
                         Wgmma<N>::mma_rs(acc, hi[k], dbh, 1);
                     }
-                }
-                wgmma_commit();
-                wgmma_wait<0>();
-                wgmma_fence_operands(acc);
+                    wgmma_commit();
+                    wgmma_wait<0>();
+                    wgmma_fence_operands(acc);
 #pragma unroll
-                for (int k = 0; k < BLOCK_KP / 8; ++k) {
-                    wgmma_fence_operands(hi[k]);
-                    wgmma_fence_operands(lo[k]);
+                    for (int k = 0; k < BLOCK_KP / 8; ++k) {
+                        wgmma_fence_operands(hi[k]);
+                        wgmma_fence_operands(lo[k]);
+                    }
                 }
                 mbar_arrive(empty(s));
                 if (++s == S) { s = 0; ph ^= 1; }
@@ -344,13 +365,18 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
                     const int h = i >> 1, chunk = i & 1;
                     if (chunk < nchunk) {
                         const uint32_t o = (uint32_t)chunk * 4u * CORE_SBO + (uint32_t)h * 512u;
-                        float hi[4], lo[4];
+                        if constexpr (SINGLE) {
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) split_tf32(v[i].v[e], hi[e], lo[e]);
+                            for (int e = 0; e < 4; ++e) st_shared_f32(t_hi + o + 16u * e, round_tf32(v[i].v[e]));
+                        } else {
+                            float hi[4], lo[4];
 #pragma unroll
-                        for (int e = 0; e < 4; ++e) {
-                            st_shared_f32(t_hi + o + 16u * e, hi[e]);
-                            st_shared_f32(t_lo + o + 16u * e, lo[e]);
+                            for (int e = 0; e < 4; ++e) split_tf32(v[i].v[e], hi[e], lo[e]);
+#pragma unroll
+                            for (int e = 0; e < 4; ++e) {
+                                st_shared_f32(t_hi + o + 16u * e, hi[e]);
+                                st_shared_f32(t_lo + o + 16u * e, lo[e]);
+                            }
                         }
                     }
                 }
@@ -372,6 +398,16 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradPar
             }
         }
     }
+}
+
+template <int PRE, bool UP, bool VEC>
+__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tc_kernel(const WgradParams p) {
+    wgrad_body<PRE, UP, VEC, false>(p);
+}
+
+template <int PRE, bool UP, bool VEC>
+__global__ void __launch_bounds__(NUM_THREADS, 1) wgrad_tf32_kernel(const WgradParams p) {
+    wgrad_body<PRE, UP, VEC, true>(p);
 }
 
 // dW[co,ci,kh,kw] (arbitrary strides) = sum_split part[split][tap][ci][co]; fixed summation order -> deterministic
@@ -496,7 +532,6 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     p.kb_per_split = (p.KBp + splitK - 1) / splitK;
     p.x_vec = bts_aligned16(x) && (x_pixel_stride % 4 == 0);
     p.dy_vec = bts_aligned16(dy) && (dy_pixel_stride % 4 == 0);
-    p.precision = precision;
     p.fd_wout = make_fastdiv((uint32_t)p.Wout);
     p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     const int taps = KH * KW;
@@ -517,7 +552,7 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     {
         const int nchunk = (p.n_tile + 31) / 32;
         p.b_bytes = nchunk * 4 * (int)CORE_SBO;
-        p.stage_bytes = X_BYTES + 2 * p.b_bytes;
+        p.stage_bytes = X_BYTES + (precision ? 1 : 2) * p.b_bytes;
         p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
         if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
         if (p.stages < 2) return BTS_EINVAL;
@@ -529,28 +564,34 @@ extern "C" int bts_conv_wgrad(const float *x, long long x_pixel_stride, int B, i
     const int pre = (pre_scale ? 2 : 0) | (p.pre_relu ? 1 : 0);
     const bool vec = p.x_vec && p.dy_vec;   // aligned bases + pixel strides % 4 == 0 (channel tails masked in-kernel)
     cudaError_t err = cudaSuccess;
-#define BTS_LAUNCH(PRE, UP, VEC)                                                                                    \
+#define BTS_LAUNCH(KERNEL, PRE, UP, VEC)                                                                            \
     do {                                                                                                            \
-        static bool attr_set_[BTS_MAX_DEVICES] = {}; bool &attr_set = attr_set_[bts_cur_device()];                                                                             \
+        static bool attr_set_[BTS_MAX_DEVICES] = {}; bool &attr_set = attr_set_[bts_cur_device()];                  \
         if (!attr_set) {                                                                                            \
-            err = cudaFuncSetAttribute(wgrad_tc_kernel<PRE, UP, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+            err = cudaFuncSetAttribute(KERNEL<PRE, UP, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
                                        SMEM_LIMIT);                                                                 \
             if (err != cudaSuccess) return (int)err;                                                                \
             attr_set = true;                                                                                        \
         }                                                                                                           \
-        wgrad_tc_kernel<PRE, UP, VEC><<<grid, NUM_THREADS, smem, st>>>(p);                                          \
+        KERNEL<PRE, UP, VEC><<<grid, NUM_THREADS, smem, st>>>(p);                                                   \
     } while (0)
-#define BTS_DISPATCH_UV(PRE)                                                                     \
-    do {                                                                                         \
-        if (p.up) { if (vec) BTS_LAUNCH(PRE, true, true); else BTS_LAUNCH(PRE, true, false); }   \
-        else { if (vec) BTS_LAUNCH(PRE, false, true); else BTS_LAUNCH(PRE, false, false); }      \
+#define BTS_DISPATCH_UV(KERNEL, PRE)                                                                                \
+    do {                                                                                                            \
+        if (p.up) { if (vec) BTS_LAUNCH(KERNEL, PRE, true, true); else BTS_LAUNCH(KERNEL, PRE, true, false); }      \
+        else { if (vec) BTS_LAUNCH(KERNEL, PRE, false, true); else BTS_LAUNCH(KERNEL, PRE, false, false); }         \
     } while (0)
-    switch (pre) {
-        case 0: BTS_DISPATCH_UV(0); break;
-        case 1: BTS_DISPATCH_UV(1); break;
-        case 2: BTS_DISPATCH_UV(2); break;
-        default: BTS_DISPATCH_UV(3); break;
-    }
+#define BTS_DISPATCH(KERNEL)                                                                                        \
+    do {                                                                                                            \
+        switch (pre) {                                                                                              \
+            case 0: BTS_DISPATCH_UV(KERNEL, 0); break;                                                              \
+            case 1: BTS_DISPATCH_UV(KERNEL, 1); break;                                                              \
+            case 2: BTS_DISPATCH_UV(KERNEL, 2); break;                                                              \
+            default: BTS_DISPATCH_UV(KERNEL, 3); break;                                                             \
+        }                                                                                                           \
+    } while (0)
+    if (precision) BTS_DISPATCH(wgrad_tf32_kernel);
+    else BTS_DISPATCH(wgrad_tc_kernel);
+#undef BTS_DISPATCH
 #undef BTS_DISPATCH_UV
 #undef BTS_LAUNCH
     BTS_LAUNCH_CHECK();
@@ -623,12 +664,11 @@ extern "C" int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, 
     p.kb_per_split = (p.KBp + splitK - 1) / splitK;
     p.x_vec = bts_aligned16(x) && (x_pixel_stride % 4 == 0);
     p.dy_vec = bts_aligned16(dy) && (dy_pixel_stride % 4 == 0);
-    p.precision = precision;
     p.fd_wout = make_fastdiv((uint32_t)p.Wout);
     p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     const int taps = KH * KW;
     p.b_bytes = 2 * 4 * (int)CORE_SBO;
-    p.stage_bytes = X_BYTES + 2 * p.b_bytes;
+    p.stage_bytes = X_BYTES + (precision ? 1 : 2) * p.b_bytes;
     p.stages = (SMEM_LIMIT - 1024 - 2 * BLOCK_CI * 4 - 256) / p.stage_bytes;
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     const int smem = p.stages * p.stage_bytes + 2 * BLOCK_CI * 4 + 256 + 1024;
@@ -637,19 +677,20 @@ extern "C" int bts_conv_wgrad_grouped(const float *x, long long x_pixel_stride, 
     cudaStream_t st = (cudaStream_t)stream;
     cudaError_t err = cudaSuccess;
     const bool vec = p.x_vec && p.dy_vec;
-#define BTS_LAUNCH_G(VEC)                                                                                            \
+#define BTS_LAUNCH_G(KERNEL, VEC)                                                                                    \
     do {                                                                                                             \
         static bool attr_set_[BTS_MAX_DEVICES] = {};                                                                 \
         bool &attr_set = attr_set_[bts_cur_device()];                                                                \
         if (!attr_set) {                                                                                             \
-            err = cudaFuncSetAttribute(wgrad_tc_kernel<0, false, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,  \
+            err = cudaFuncSetAttribute(KERNEL<0, false, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize,           \
                                        SMEM_LIMIT);                                                                  \
             if (err != cudaSuccess) return (int)err;                                                                 \
             attr_set = true;                                                                                         \
         }                                                                                                            \
-        wgrad_tc_kernel<0, false, VEC><<<grid, NUM_THREADS, smem, st>>>(p);                                          \
+        KERNEL<0, false, VEC><<<grid, NUM_THREADS, smem, st>>>(p);                                                   \
     } while (0)
-    if (vec) BTS_LAUNCH_G(true); else BTS_LAUNCH_G(false);
+    if (precision) { if (vec) BTS_LAUNCH_G(wgrad_tf32_kernel, true); else BTS_LAUNCH_G(wgrad_tf32_kernel, false); }
+    else { if (vec) BTS_LAUNCH_G(wgrad_tc_kernel, true); else BTS_LAUNCH_G(wgrad_tc_kernel, false); }
 #undef BTS_LAUNCH_G
     BTS_LAUNCH_CHECK();
     const long long total = (long long)taps * width * cpg;

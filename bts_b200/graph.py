@@ -7,6 +7,9 @@ capturable: no host synchronisation, allocations through torch's caching allocat
 statistics and `num_batches_tracked` updated by device ops, packed conv operators re-written IN PLACE by
 bts_b200.optim.FusedAdamW after each step.  One replay = one step's forward + loss + backward; the gradients land in static
 `.grad` tensors that the (eager) collective and optimizer step then read.
+
+The numeric mode of the tensor-core engine (bts_b200.set_precision) is resolved when each launch is enqueued, so a graph
+replays the mode it was captured in, whatever the mode is at replay time.  Capture a new GraphedTrainStep after switching.
 """
 import torch
 

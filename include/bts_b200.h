@@ -88,7 +88,9 @@ int bts_plane_head_bwd(const float *d_scaled, const float *d_ds, const float *c3
 
 /* ---- wgmma implicit-GEMM convolution (pytorch/bts.py:51-80,153-194; torchvision dense/bottleneck layers) ----
  * NHWC activations, fp32 in / fp32 out, parity-grade 3xTF32 on the Hopper tensor cores (precision=0) or
- * single-pass TF32 (precision=1, labelled fast mode, not parity).
+ * single-pass TF32 (precision=1, opt-in, not parity).  precision=1 launches the dedicated single-pass kernels
+ * (conv_tf32_kernel, wgrad_tf32_kernel, wgrad2_tf32_kernel): one product per k8 step, and shared-memory stages that hold
+ * only the hi half of the weight / dY operand.  The packed weights are the same for both values.
  *   out[p,co] = act( sum_{tap,ci} pre(x[p (+) tap, ci]) * w[co,ci,tap] )
  *   pre : x*pre_scale[ci]+pre_shift[ci] (folded BatchNorm; both NULL to skip), then ReLU if pre_relu;
  *         zero padding is applied after pre.  upsample2=1 folds a nearest x2 up-sample of the source in.
