@@ -80,6 +80,9 @@ SIGNATURES = {
     "bts_conv_fwd_stats": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p, _p, _p],
     "bts_conv_fwd_ex": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p,
                         _p, _p],
+    "bts_conv_fwd_splitk_plan": [_i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
+    "bts_conv_fwd_splitk": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i,
+                            _p, _p, _i, _p, _p],
     "bts_conv_fwd_bnbwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _ll, _i, _p, _ll, _p, _i,
                            _p, _p, _p],
     "bts_bn_bwd_coef": [_p, _p, _ll, _i, _p, _p, _p, _p, _p],

@@ -10,6 +10,7 @@ fp32-grade; "tf32" runs the single-pass TF32 kernels, one product per MMA.  Only
 follow the mode; the CUDA-core kernels (narrow 1x1 and Cout = 1 heads, depthwise, BatchNorm, LPG, loss, optimizer) and
 the library-conv fallback compute in fp32 either way, and their routing does not depend on it.
 """
+import contextlib
 import ctypes
 import weakref
 
@@ -26,6 +27,36 @@ PW_WGRAD = True                                               # CUDA-core wgrad 
 PW_MIN_PIXELS = 200000                                        # below this the tensor-core path is already short
 TRACE = _os.environ.get("BTS_B200_TRACE", "0") == "1"     # per-call CUDA-event timing, aggregated by shape
 trace_log = []
+SPLITK = True                 # split-K forward launches inside inference(); tools and tests turn it off to compare
+_inference_depth = 0
+_splitk_plans = {}            # (device, launch geometry, requested splits) -> (splits, workspace floats)
+
+
+@contextlib.contextmanager
+def inference():
+    """Scope in which no backward pass follows the forward launches: conv2d_tc may then cut a launch whose tiles fill at
+    most half the SMs (batch-1 maps) into split-K ranges, whose partial sums a second kernel adds.  BtsModel.forward enters
+    it under torch.no_grad() or when nothing requires grad; enter it directly when calling the engine below the model.
+    Launches with epilogue statistics or BatchNorm-backward sums (training) never split, inside the scope or not."""
+    global _inference_depth
+    _inference_depth += 1
+    try:
+        yield
+    finally:
+        _inference_depth -= 1
+
+
+def splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Cout, splits=0):
+    """(splits, workspace floats) of a forward / dgrad engine launch on the current device: splits = 0 asks for the engine's
+    choice (1: no split), n > 0 forces n (reduced so that no split is empty)"""
+    key = (torch.cuda.current_device(), B, Hout, Wout, kwin, Cin, KH, KW, Cout, splits)
+    plan = _splitk_plans.get(key)
+    if plan is None:
+        n, wsf = ctypes.c_int(int(splits)), ctypes.c_longlong(0)
+        _lib.check(_lib.lib().bts_conv_fwd_splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Cout, ctypes.byref(n),
+                                                        ctypes.byref(wsf)), "bts_conv_fwd_splitk_plan")
+        plan = _splitk_plans[key] = (n.value, wsf.value)
+    return plan
 
 
 PRECISIONS = {"fp32": 0, "tf32": 1}       # mode -> the `precision` argument of the C ABI
@@ -160,6 +191,31 @@ def repack_cached():
     return len(live)
 
 
+def cached_operators(params):
+    """the cache entries [(key, entry)] of the packed operators of `params` -- the buffers a CUDA graph captured over
+    these parameters reads (bts_b200.graph.GraphedInference keeps them)"""
+    ids = {id(p) for p in params}
+    return [(k, e) for k, e in _pack_cache.items() if k[0] in ids and e[0]() is not None]
+
+
+def restore_operators(entries):
+    """Puts the packed operators `entries` (from cached_operators) back into the cache wherever a later pack_weights
+    replaced them or invalidate_packed() dropped them, marked stale, so that the next repack_cached() rewrites those very
+    buffers in place.  Returns True if any was put back.
+
+    The cache is shared by eager forwards and captured graphs: a buffer that an eager pack_weights made after the weights
+    changed is dropped here (freed once no pending work uses it), and eager forwards then read the graph's buffers, which
+    repack_cached() keeps current.  repack_cached() rewrites every live cached operator, of every model, in its one
+    launch -- not only the graph's."""
+    put = False
+    for k, (ref, ver, ptr, packed, groups) in entries:
+        cur = _pack_cache.get(k)
+        if cur is None or cur[3] is not packed:
+            _pack_cache[k] = (ref, -1, ptr, packed, groups)
+            put = True
+    return put
+
+
 def group_window(width, cpg):
     return _lib.lib().bts_conv_group_window(int(width), int(cpg))
 
@@ -215,7 +271,7 @@ def _nhwc_view(x):
 
 def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_shift=None, pre_relu=False,
               upsample2=False, act=None, out=None, precision=None, packed=None, cout=None, transpose_flip=False,
-              stats=None, groups=1, zero_stuff_out=None, bn_bwd=None):
+              stats=None, groups=1, zero_stuff_out=None, bn_bwd=None, splits=None):
     """Runs the engine.  x: (B,Cin,Hs,Ws) NHWC-in-memory fp32 CUDA.  Returns (B,Cout,Hout,Wout) channels_last.
     `out` may be a pre-allocated channels_last tensor or a channel slice of one (concat-free writes).
     `stats`: a ZEROED fp64 [2, Cout] tensor that receives per-channel (sum, sum of squares) of the output, reduced in the
@@ -227,7 +283,9 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
     `groups` > 1: block-diagonal operator (ResNeXt 3x3).  `zero_stuff_out=(H,W)`: x is the gradient of a stride-2 layer
     whose input was HxW -- the source is read as its zero-stuffed x2 expansion (use with transpose_flip, stride 1).
     `precision`: None = the mode of set_precision, 0 = 3xTF32, 1 = single-pass TF32 on the engine (an explicit 1 also
-    keeps the layer off the CUDA-core 1x1 kernel, which is fp32 in every mode)."""
+    keeps the layer off the CUDA-core 1x1 kernel, which is fp32 in every mode).
+    Inside `inference()` a launch without `stats` / `bn_bwd` runs split-K when the engine's plan says so.  `splits` (tests)
+    forces a split count on the engine path: 1 never splits, n > 1 always does (and rejects `stats` / `bn_bwd`)."""
     _need_cuda(x, weight)
     if x.dtype != torch.float32:
         raise TypeError("conv2d_tc computes in fp32 (3xTF32 on wgmma); got %s" % x.dtype)
@@ -246,7 +304,7 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         raise ValueError("weight expects %d input channels, got %d" % (Ci, Cin))
     if (PW_FWD and KH == 1 and KW == 1 and stride == 1 and padding == 0 and groups == 1 and not upsample2
             and zero_stuff_out is None and pre_scale is None and not pre_relu and stats is None and bn_bwd is None
-            and precision in (None, 0) and packed is None and act in ACT and B * Hs * Ws >= PW_MIN_PIXELS
+            and precision in (None, 0) and packed is None and splits is None and act in ACT and B * Hs * Ws >= PW_MIN_PIXELS
             and xs % 4 == 0 and x.data_ptr() % 16 == 0 and _lib.lib().bts_conv_pw_fwd_eligible(Cin, Co)):
         # narrow 1x1 layers of the reduction heads (forward and dgrad): HBM-bound CUDA-core kernel (csrc/pointwise.cu)
         if out is None:
@@ -296,6 +354,14 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         pre_shift = pre_shift.contiguous()
     if stats is not None and (stats.dtype != torch.float64 or tuple(stats.shape) != (2, Co) or not stats.is_contiguous()):
         raise ValueError("stats must be a contiguous fp64 [2, Cout] tensor")
+    nsplit, ws = 1, None
+    if splits is not None or (SPLITK and _inference_depth > 0 and stats is None and bn_bwd is None):
+        if bn_bwd is not None and splits > 1:
+            raise ValueError("split-K launches have no BatchNorm-backward epilogue")
+        with torch.cuda.device(x.device):
+            nsplit, wsf = splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Co, 0 if splits is None else int(splits))
+        if nsplit > 1:
+            ws = torch.empty(wsf, device=x.device, dtype=torch.float32)
     if bn_bwd is not None:
         xb, st, relu = bn_bwd
         xb, xbs = _nhwc_view(xb)
@@ -314,20 +380,28 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
         _lib.check(rc, "bts_conv_fwd_bnbwd")
         _lib.count()
         return out
+    st0 = _ptr(stats[0]) if stats is not None else None
+    st1 = _ptr(stats[1]) if stats is not None else None
     with torch.cuda.device(x.device):
-        call = lambda: _lib.lib().bts_conv_fwd_ex(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
-                                                  Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding, dilation,
-                                                  _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift), int(pre_relu),
-                                                  _ptr(out), os_, ACT[act], int(precision),
-                                                  _ptr(stats[0]) if stats is not None else None,
-                                                  _ptr(stats[1]) if stats is not None else None, _stream())
+        if ws is not None:
+            call = lambda: _lib.lib().bts_conv_fwd_splitk(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
+                                                          Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding,
+                                                          dilation, _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift),
+                                                          int(pre_relu), _ptr(out), os_, ACT[act], int(precision), st0, st1,
+                                                          nsplit, _ptr(ws), _stream())
+        else:
+            call = lambda: _lib.lib().bts_conv_fwd_ex(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
+                                                      Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding, dilation,
+                                                      _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift), int(pre_relu),
+                                                      _ptr(out), os_, ACT[act], int(precision), st0, st1, _stream())
         rc = _traced("dgrad" if transpose_flip else "fwd",
-                     "%dx%dx%d %d->%d k%d d%d s%d%s%s" % (B, Hs, Ws, Cin, Co, KH, dilation, stride,
-                                                         " up" if upsample2 else (" zs" if mode == 2 else ""),
-                                                         " g%d" % groups if groups > 1 else ""),
+                     "%dx%dx%d %d->%d k%d d%d s%d%s%s%s" % (B, Hs, Ws, Cin, Co, KH, dilation, stride,
+                                                           " up" if upsample2 else (" zs" if mode == 2 else ""),
+                                                           " g%d" % groups if groups > 1 else "",
+                                                           " sk%d" % nsplit if ws is not None else ""),
                      call, 2.0 * B * Hout * Wout * Co * (Cin // groups) * KH * KW / (4.0 if mode == 2 else 1.0))
-    _lib.check(rc, "bts_conv_fwd_ex")
-    _lib.count()
+    _lib.check(rc, "bts_conv_fwd_splitk" if ws is not None else "bts_conv_fwd_ex")
+    _lib.count(2 if ws is not None else 1)
     return out
 
 

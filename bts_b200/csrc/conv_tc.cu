@@ -97,6 +97,14 @@ struct ConvParams {
     int bnb_relu;
     int stages, stage_bytes; // smem ring: as many (A + B hi/lo, single pass: A + B hi) stages as fit
     tc::FastDiv fd_wout, fd_hout, fd_ntiles;
+    // split-K: the grid is splits x vgrid CTAs; CTA b runs split s = b / vgrid over tiles b - s * vgrid, + vgrid, ... and
+    // streams the kb_split k-blocks [s * kb_split, (s + 1) * kb_split) of each; its epilogue stores the raw tile sum at
+    // out + s * split_stride (the workspace).  The last split's k-blocks past KB lie past the last tap: their A tile is
+    // zero-filled like any quad past the last tap and their weight tile index is clamped to w_last (finite values times
+    // zeros leave the tile sum unchanged).  Without split-K: splits = 1, vgrid = the grid, kb_split = KB, split_stride = 0.
+    int splits, kb_split, vgrid, w_last;
+    long long split_stride;
+    tc::FastDiv fd_vgrid;
 };
 
 using namespace tc;
@@ -241,8 +249,20 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
     const int KB = p.KB;
     if (p.stat_sum)
         for (int i = threadIdx.x; i < STAT_SETS * 2 * n_tile; i += NUM_THREADS) s_stat[i] = 0.0;
-    // tiles of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...   (tile -> m_tile = tile / n_tiles, nt = tile % n_tiles)
-    const int my_tiles = (p.total_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+    // tiles of this CTA: t0, t0 + vgrid, ...   (tile -> m_tile = tile / n_tiles, nt = tile % n_tiles), all of split s.
+    // s and t0 are recomputed from %ctaid where they are used (volatile: not hoisted), so they hold no register across
+    // the k-block loops, where the producers have none to spare.
+    auto cta_split = [&]() {
+        uint32_t b;
+        asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+        return (int)fdiv(b, p.fd_vgrid);
+    };
+    auto cta_tile0 = [&]() {
+        uint32_t b;
+        asm volatile("mov.u32 %0, %%ctaid.x;" : "=r"(b));
+        return (int)b - (int)fdiv(b, p.fd_vgrid) * p.vgrid;
+    };
+    const int my_tiles = (p.total_tiles - cta_tile0() + p.vgrid - 1) / p.vgrid;
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < S; ++s) {
@@ -266,7 +286,7 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
         // The group that fills a k-block also stages its weight tile: right after the stage has been released, one lane
         // issues the 1-D bulk async copy (cp.async.bulk) of the pre-packed, pre-split, pre-swizzled B hi/lo rows,
         // completing on an mbarrier.
-        const int total_kb = my_tiles * KB;        // host guarantees < 2^31
+        const int total_kb = my_tiles * p.kb_split;        // host guarantees < 2^31
         const int pt = threadIdx.x - CONSUMER_THREADS;
         const int grp = pt / PRODUCER_THREADS;     // producer group: global k-blocks gk == grp (mod 2)
         const int t = pt % PRODUCER_THREADS;
@@ -285,20 +305,22 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
         const float *__restrict__ xg = p.x;
         // swizzled byte offset of (row r0 + 16 i, chunk) inside a tile = roff0 + i * 2048
         const uint32_t roff0 = (uint32_t)r0 * 128u + (uint32_t)((chunk ^ (r0 & 7)) << 4);
+        const int gq0 = chunk + 8 * p.kb_split * cta_split();    // this lane's channel quad in the split's first k-block
         // ---- cursor: (tile iteration, k-block in tile) of the next k-block this group fills; this lane's channel quad of
         //      that k-block is g = 8 kb + chunk -> (tap, quad in tap) by multiply-shift division
         // oyx[i]: the row's top-left source coordinate, (oy << 16) | (ox & 0xffff) -- one register per row instead of two
         // (host: |coordinates| < 2^14)
         int oyx[8], rowoff[8];
-        int l_ti = 0, l_kb = grp, cur_ti = -1, cur_nt = 0;      // (KB may be 1)
-        while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
+        // l_kb counts the k-blocks of the split (kb_split per tile); cur_w = the weight tile of the split's first k-block
+        int l_ti = 0, l_kb = grp, cur_ti = -1, cur_w = 0;       // (kb_split may be 1)
+        while (l_kb >= p.kb_split) { l_kb -= p.kb_split; ++l_ti; }
         auto set_tile = [&](int ti) {
             cur_ti = ti;
-            const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+            const int tile = cta_tile0() + ti * p.vgrid;
             const uint32_t m_tile = fdiv((uint32_t)tile, p.fd_ntiles);
             const uint32_t m_base = m_tile * BLOCK_M + (uint32_t)r0;
             const int nt = tile - (int)m_tile * p.n_tiles;
-            cur_nt = nt;
+            cur_w = nt * KB + p.kb_split * cta_split();
             const int cwin = p.kwin ? nt * p.n_tile / p.kwin * p.kwin : 0;     // first input channel of this n-tile's window
 #pragma unroll
             for (int i = 0; i < 8; ++i) {
@@ -366,8 +388,8 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
 #pragma unroll 1
         for (int it = 0; it < mine; ++it) {
             if (l_ti != cur_ti) set_tile(l_ti);
-            const int w = cur_nt * KB + l_kb;      // the k-block's weight tile in wpack (host guarantees < 2^31)
-            const uint32_t g = (uint32_t)(l_kb * 8 + chunk);
+            const int w = min(cur_w + l_kb, p.w_last);   // the k-block's weight tile in wpack (host guarantees < 2^31)
+            const uint32_t g = (uint32_t)(l_kb * 8 + gq0);
             const uint32_t tap = fdiv(g, p.fd_cq);
             const uint32_t ky = fdiv(tap, p.fd_kw);
             const int kx = (int)(tap - ky * (uint32_t)KW);
@@ -423,7 +445,7 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
             s_s += 2;
             if (s_s >= S) { s_s -= S; s_ph ^= 1; }
             l_kb += 2;
-            while (l_kb >= KB) { l_kb -= KB; ++l_ti; }
+            while (l_kb >= p.kb_split) { l_kb -= p.kb_split; ++l_ti; }
         }
         if (PRE != 0 && pend_s >= 0) {
             cp_async_wait_dyn(0);
@@ -461,11 +483,11 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
             uint32_t aF = aF0;
             uint64_t d = dB0;
             for (int ti = 0; ti < my_tiles; ++ti) {
-                const int tile = (int)blockIdx.x + ti * (int)gridDim.x;
+                const int tile = cta_tile0() + ti * p.vgrid;
                 const int m_tile = (int)fdiv((uint32_t)tile, p.fd_ntiles), nt = tile - m_tile * p.n_tiles;
 #pragma unroll
                 for (int i = 0; i < R; ++i) tot[i] = 0.f;
-                for (int kb = 0; kb < KB; ++kb) {
+                for (int kb = 0; kb < p.kb_split; ++kb) {
                     mbar_wait_no_trap(full(s), ph);
                     if constexpr (SINGLE) {
                         uint32_t hi[BLOCK_K / 8][4];
@@ -531,8 +553,9 @@ __device__ __forceinline__ void conv_body(const ConvParams &p) {
                 const float *bnb_x = p.bnb_x, *bnb_st = p.bnb_st;
                 asm volatile("" : "+r"(cq), "+r"(Cout), "+l"(bnb_x), "+l"(bnb_st));
                 const long long m0 = (long long)m_tile * BLOCK_M + row, m1 = m0 + 8;
-                float *orow0 = p.out + (m0 < p.M ? m0 : 0) * p.os + (long long)nt * n_tile;
-                float *orow1 = p.out + (m1 < p.M ? m1 : 0) * p.os + (long long)nt * n_tile;
+                float *out = p.out + cta_split() * p.split_stride;       // split-K: this split's slice of the workspace
+                float *orow0 = out + (m0 < p.M ? m0 : 0) * p.os + (long long)nt * n_tile;
+                float *orow1 = out + (m1 < p.M ? m1 : 0) * p.os + (long long)nt * n_tile;
 #pragma unroll
                 for (int j = 0; j < N / 8; ++j) {
                     const int col = 8 * j + cq;
@@ -660,6 +683,42 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tf32_kernel(const ConvPar
     conv_body<PRE, UP, VEC, true>(p);
 }
 
+__device__ __forceinline__ float splitk_act(float a, int act) {      // the activations of conv_body's epilogue
+    if (act == 1) return a > 0.f ? a : expm1f(a);
+    if (act == 2) return 1.0f / (1.0f + expf(-a));
+    return a;
+}
+
+// Split-K reduction: out[m, c] = act(part[0][m][c] + part[1][m][c] + ...) for c < Cout, the splits added in a fixed order
+// (bit-reproducible run to run); part is [splits][M][Cpad] with Cpad = Cout rounded up to 4, out is NHWC at pixel stride
+// os (a channel slice of a wider slab is fine).  One thread per 16-byte channel quad of a pixel; n = M * Cpad / 4 < 2^31.
+// 256-thread blocks; the grid stride is written with the literal block size (with blockDim.x ptxas keeps it on a stack
+// frame).
+__global__ void __launch_bounds__(256) conv_splitk_reduce_kernel(const float *__restrict__ part, int splits,
+                                                                 long long split_stride, int n, int Cout, int Cpad, int act,
+                                                                 float *__restrict__ out, long long os, int vec) {
+    const int CQ = Cpad >> 2;
+    for (int i = (int)blockIdx.x * 256 + (int)threadIdx.x; i < n; i += (int)gridDim.x * 256) {
+        const int m = i / CQ, c = (i - m * CQ) * 4;
+        const float *src = part + (long long)m * Cpad + c;
+        float4 a = __ldg(reinterpret_cast<const float4 *>(src));
+        for (int s = 1; s < splits; ++s) {
+            const float4 b = __ldg(reinterpret_cast<const float4 *>(src + s * split_stride));
+            a.x += b.x; a.y += b.y; a.z += b.z; a.w += b.w;
+        }
+        a.x = splitk_act(a.x, act); a.y = splitk_act(a.y, act); a.z = splitk_act(a.z, act); a.w = splitk_act(a.w, act);
+        float *dst = out + (long long)m * os + c;
+        if (vec && c + 4 <= Cout) {
+            *reinterpret_cast<float4 *>(dst) = a;
+        } else {
+            dst[0] = a.x;
+            if (c + 1 < Cout) dst[1] = a.y;
+            if (c + 2 < Cout) dst[2] = a.z;
+            if (c + 3 < Cout) dst[3] = a.w;
+        }
+    }
+}
+
 }  // namespace
 
 // ------------------------------------------------------------------------------------------- C ABI
@@ -758,7 +817,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
                          int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                          const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
                          long long out_pixel_stride, int act, int precision, double *stat_sum, double *stat_sumsq,
-                         void *stream, const BnBwdArgs *bnb = nullptr) {
+                         void *stream, const BnBwdArgs *bnb = nullptr, int splits = 1, float *workspace = nullptr) {
     if (!x || !wpack || !out || B < 0 || Hs < 1 || Ws < 1 || Cin < 1 || Cout < 1 || KH < 1 || KW < 1 || stride < 1 ||
         pad < 0 || dil < 1)
         return BTS_EINVAL;
@@ -769,6 +828,9 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     if (upsample2 == 2 && (stride != 1 || out_h < 1 || out_w < 1)) return BTS_EINVAL;
     if (kwin && (pre_scale || Cin % kwin || Cout % kwin)) return BTS_EINVAL;   // whole windows; no pre-op on grouped convs
     if (!bts_aligned16(wpack)) return BTS_EALIGN;
+    const bool split_mode = workspace != nullptr;
+    if (split_mode && (splits < 1 || stat_sum || stat_sumsq || bnb)) return BTS_EINVAL;   // raw sums: no epilogue reductions
+    if (split_mode && !bts_aligned16(workspace)) return BTS_EALIGN;
     if (B == 0) return 0;
     if ((long long)B * Hs * Ws * x_pixel_stride >= 0x7fffffffLL) return BTS_EINVAL;   // 32-bit element offsets
     ConvParams p;
@@ -809,6 +871,21 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     if (m_tiles * p.n_tiles * (long long)p.KB > 0x7fffffffLL || p.M + BLOCK_M >= 0x7fffffffLL) return BTS_EINVAL;
     p.m_tiles = (int)m_tiles;
     p.total_tiles = (int)(m_tiles * p.n_tiles);
+    const int sms = bts_num_sms();
+    // split-K: ranges of kb_split k-blocks (the last one padded past KB); a count that would leave a split empty is reduced
+    p.kb_split = (p.KB + splits - 1) / splits;
+    p.splits = split_mode ? (p.KB + p.kb_split - 1) / p.kb_split : 1;
+    if (!split_mode) p.kb_split = p.KB;
+    if (p.splits > sms) return BTS_EINVAL;
+    p.vgrid = p.total_tiles < sms / p.splits ? p.total_tiles : sms / p.splits;
+    p.fd_vgrid = make_fastdiv((uint32_t)p.vgrid);
+    p.w_last = p.n_tiles * p.KB - 1;
+    const int Cpad = (Cout + 3) / 4 * 4;
+    p.split_stride = 0;
+    if (split_mode) {
+        if (p.M * (Cpad / 4) >= 0x7fffffffLL) return BTS_EINVAL;
+        p.out = workspace; p.os = Cpad; p.act = 0; p.split_stride = p.M * Cpad;
+    }
     p.fd_wout = make_fastdiv((uint32_t)p.Wout);
     p.fd_hout = make_fastdiv((uint32_t)p.Hout);
     p.fd_ntiles = make_fastdiv((uint32_t)p.n_tiles);
@@ -821,8 +898,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     if (p.stages > MAX_STAGES) p.stages = MAX_STAGES;
     if (p.stages < 2) return BTS_EINVAL;
     const int smem = p.stages * p.stage_bytes + pre_bytes + BAR_BYTES + stat_bytes + 1024;
-    const int sms = bts_num_sms();
-    dim3 grid((unsigned)(p.total_tiles < sms ? p.total_tiles : sms));
+    dim3 grid((unsigned)(p.vgrid * p.splits));
     const bool vec = p.vec_ok;      // aligned base + pixel stride % 4 == 0 (a channel tail is masked in-kernel)
     cudaError_t err = cudaSuccess;
 #define BTS_LAUNCH(KERNEL, PRE, UP, VEC)                                                                           \
@@ -858,6 +934,15 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
 #undef BTS_DISPATCH_UV
 #undef BTS_LAUNCH
     BTS_LAUNCH_CHECK();
+    if (split_mode) {
+        const int n = (int)(p.M * (Cpad / 4));
+        int rgrid = (n + 255) / 256;
+        if (rgrid > sms * 8) rgrid = sms * 8;
+        const int vec = bts_aligned16(out) && out_pixel_stride % 4 == 0;
+        conv_splitk_reduce_kernel<<<rgrid, 256, 0, (cudaStream_t)stream>>>(workspace, p.splits, p.split_stride, n, Cout,
+                                                                           Cpad, act, out, out_pixel_stride, vec);
+        BTS_LAUNCH_CHECK();
+    }
     return 0;
 }
 
@@ -895,6 +980,58 @@ extern "C" int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, 
     return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
                          Cout, pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq,
                          stream);
+}
+
+// Split-K plan of a forward / dgrad launch (see bts_b200.h).  A launch splits only when its tiles fill at most half the SMs:
+// splits = as many as keep tiles * splits within one wave of bts_num_sms() and every split at least SPLITK_MIN_KB k-blocks
+// long (its padded tail included), so that each tile of a split streams more k-blocks than the deepest stage ring holds
+// (MAX_STAGES) and its epilogue, which writes the partial tile sum, stays short next to its main loop.  *splits > 0 on
+// entry forces that count instead.
+constexpr int SPLITK_MIN_KB = 8;
+static_assert(SPLITK_MIN_KB > MAX_STAGES, "a split must stream more k-blocks than the ring holds");
+
+extern "C" int bts_conv_fwd_splitk_plan(int B, int Hout, int Wout, int kwin, int Cin, int KH, int KW, int Cout, int *splits,
+                                        long long *workspace_floats) {
+    if (!splits || !workspace_floats || B < 1 || Hout < 1 || Wout < 1 || kwin < 0 || kwin % 16 || Cin < 1 || Cout < 1 ||
+        KH < 1 || KW < 1 || *splits < 0)
+        return BTS_EINVAL;
+    const int n_tile = kwin ? bts_conv_group_n_tile(kwin) : bts_conv_n_tile(Cout);
+    if (!n_tile) return BTS_EINVAL;
+    const long long n_tiles = (Cout + n_tile - 1) / n_tile;
+    const long long M = (long long)B * Hout * Wout;
+    const long long tiles = (M + BLOCK_M - 1) / BLOCK_M * n_tiles;
+    const long long KB = ((long long)KH * KW * (((kwin ? kwin : Cin) + 3) / 4) + 7) / 8;
+    const long long Cpad = (Cout + 3) / 4 * 4;
+    const long long sms = bts_num_sms();
+    long long s = *splits;
+    if (s == 0) {
+        s = 1;
+        if (2 * tiles <= sms) {
+            s = sms / tiles;
+            if (s > KB / SPLITK_MIN_KB) s = KB / SPLITK_MIN_KB;
+        }
+        if (M * (Cpad / 4) >= 0x7fffffffLL) s = 1;
+    }
+    if (s > KB) s = KB;
+    if (s > sms) s = sms;
+    if (s > 1) s = (KB + (KB + s - 1) / s - 1) / ((KB + s - 1) / s);       // no empty split (as the launch counts them)
+    if (s < 1) s = 1;
+    *splits = (int)s;
+    *workspace_floats = s > 1 ? s * M * Cpad : 0;
+    return 0;
+}
+
+// bts_conv_fwd_ex in split-K mode (see bts_b200.h): the conv kernel writes raw partial tile sums into `workspace`
+// ([splits][M][Cpad]), conv_splitk_reduce_kernel adds them and applies the activation into out.
+extern "C" int bts_conv_fwd_splitk(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h,
+                                   int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
+                                   const float *wpack, int Cout, const float *pre_scale, const float *pre_shift, int pre_relu,
+                                   float *out, long long out_pixel_stride, int act, int precision, double *stat_sum,
+                                   double *stat_sumsq, int splits, float *workspace, void *stream) {
+    if (!workspace) return BTS_EINVAL;
+    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
+                         Cout, pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq,
+                         stream, nullptr, splits, workspace);
 }
 
 // descs: device array of n PackDesc (layout above; built by the host side once per model), total = sum of packed_floats / 2

@@ -28,6 +28,13 @@ def eligible(x):
     return x.is_cuda and x.dtype == torch.float32 and x.dim() == 4
 
 
+def no_backward(x, module):
+    """True when no backward pass can follow module(x): grad mode is off, or neither x nor any parameter of `module` requires
+    grad.  Decided before an autograd Function runs: inside it, needs_input_grad reflects requires_grad alone and ignores
+    no_grad / inference_mode."""
+    return not (torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in module.parameters())))
+
+
 def _nhwc(t):
     """(tensor, pixel stride) with NHWC memory; converts (one copy) when the layout is something else"""
     return conv._nhwc_view(t)
@@ -482,9 +489,7 @@ def inverted_residual(x, block):
         dw, proj, bn3 = layers
         w1 = g1 = b1 = bn1 = None
     bn2 = dw[1]
-    # BN2 on folded running statistics can run as the depthwise conv's epilogue only when no backward follows.  That is
-    # decided here: inside the Function, needs_input_grad reflects requires_grad alone and ignores no_grad / inference_mode.
-    fuse_eval = not bn_uses_batch_stats(bn2) and not (
-        torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in block.parameters())))
+    # BN2 on folded running statistics can run as the depthwise conv's epilogue only when no backward follows
+    fuse_eval = not bn_uses_batch_stats(bn2) and no_backward(x, block)
     return _InvertedResidual.apply(x, w1, g1, b1, dw[0].weight, bn2.weight, bn2.bias, proj.weight, bn3.weight, bn3.bias,
                                    (bn1, bn2, bn3), int(dw[0].stride[0]), bool(block.use_res_connect), fuse_eval)

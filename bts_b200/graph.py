@@ -8,8 +8,12 @@ statistics and `num_batches_tracked` updated by device ops, packed conv operator
 bts_b200.optim.FusedAdamW after each step.  One replay = one step's forward + loss + backward; the gradients land in static
 `.grad` tensors that the (eager) collective and optimizer step then read.
 
+GraphedInference does the same for the batch-1 eval forward (bts_test.py, online eval): one replay = one model(x, focal)
+in eval mode under no_grad (split-K engine launches included, conv.inference()), several hundred native launches without
+their Python and ctypes cost.
+
 The numeric mode of the tensor-core engine (bts_b200.set_precision) is resolved when each launch is enqueued, so a graph
-replays the mode it was captured in, whatever the mode is at replay time.  Capture a new GraphedTrainStep after switching.
+replays the mode it was captured in, whatever the mode is at replay time.  Capture a new graph after switching.
 """
 import torch
 
@@ -57,3 +61,69 @@ class GraphedTrainStep:
         self.graph.replay()
         _lib.count(self.launches_per_replay)
         return self.loss
+
+
+class GraphedInference:
+    """model(x, focal) of an eval-mode model under torch.no_grad(), captured for one input shape into one CUDA graph.
+
+    __call__(x, focal) copies the inputs into the graph's static buffers, replays and returns the graph's static 5-tuple of
+    outputs: the next call overwrites it, so clone what has to outlive it.  The graph replays the precision mode
+    (bts_b200.set_precision) it was captured in.
+
+    Weights may change between calls (online eval during training: optimizer steps, load_state_dict): BatchNorm running
+    statistics are folded inside the graph and the CUDA-core kernels read the parameters themselves, so replays see
+    their current values; the engine reads packed operators, which are re-packed in place (one launch) before a replay
+    when a parameter's version counter moved.  In-place writes through `.data` do not move it: call
+    bts_b200.conv.invalidate_packed() after those.  A parameter or buffer whose storage was replaced (`p.data = ...`,
+    `.to()`) cannot be followed by the graph: the call raises and a new capture is needed."""
+
+    def __init__(self, model, x, focal, warmup=2):
+        from . import _lib, conv
+        if model.training:
+            raise ValueError("GraphedInference captures the eval forward: call model.eval() first")
+        self.model = model
+        self.x = x.clone()
+        self.focal = focal.clone()
+        cur = torch.cuda.current_stream()
+        side = torch.cuda.Stream()
+        side.wait_stream(cur)
+        with torch.no_grad():
+            with torch.cuda.stream(side):                  # warm-up off the capturing stream: packs every operator
+                for _ in range(warmup):
+                    model(self.x, self.focal)
+            cur.wait_stream(side)
+            torch.cuda.synchronize()
+            l0 = _lib.launches
+            self.graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(self.graph):
+                self.out = model(self.x, self.focal)
+        self.launches_per_replay = _lib.launches - l0
+        self.params = list(model.parameters())
+        self.tensors = [(t, t.data_ptr()) for t in self.params + list(model.buffers())]
+        self.versions = [p._version for p in self.params]
+        self.operators = conv.cached_operators(self.params)
+
+    def _refresh(self):
+        from . import conv
+        for t, ptr in self.tensors:
+            if t.data_ptr() != ptr:
+                raise RuntimeError("GraphedInference: a parameter or buffer of the model was re-allocated since the capture "
+                                   "(its storage moved); capture a new GraphedInference")
+        versions = [p._version for p in self.params]
+        if conv.restore_operators(self.operators) or versions != self.versions:
+            conv.repack_cached()
+            self.versions = versions
+
+    def __call__(self, x, focal):
+        from . import _lib
+        if x.shape != self.x.shape or focal.shape != self.focal.shape:
+            raise ValueError("GraphedInference was captured for x %s, focal %s; got %s, %s" % (
+                tuple(self.x.shape), tuple(self.focal.shape), tuple(x.shape), tuple(focal.shape)))
+        self._refresh()
+        if x.data_ptr() != self.x.data_ptr():
+            self.x.copy_(x, non_blocking=True)
+        if focal.data_ptr() != self.focal.data_ptr():
+            self.focal.copy_(focal, non_blocking=True)
+        self.graph.replay()
+        _lib.count(self.launches_per_replay)
+        return self.out

@@ -132,6 +132,21 @@ int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int
                     int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
                     const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
                     int act, int precision, double *stat_sum, double *stat_sumsq, void *stream);
+/* Split-K form of bts_conv_fwd_ex, for launches whose tiles (128-pixel x n-tile output blocks) leave SMs idle (batch-1
+ * inference): each tile's K range is cut into `splits` ranges run by separate CTAs, which write raw fp32 partial tile sums
+ * into `workspace` ([splits][M][Cout rounded up to 4], 16-byte aligned); a second kernel adds them in a fixed order (the
+ * result is reproducible run to run) and applies `act` into out.  stat_sum / stat_sumsq must be NULL (BTS_EINVAL
+ * otherwise): the split kernel has no statistics or BatchNorm-backward epilogue.
+ *   bts_conv_fwd_splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Cout, &splits, &workspace_floats): with *splits = 0 on
+ *   entry, the engine's choice (1 = do not split: the launch already fills more than half the SMs, or K is too short);
+ *   with *splits = n > 0, n reduced so that no split is empty.  *workspace_floats: the workspace that count needs. */
+int bts_conv_fwd_splitk_plan(int B, int Hout, int Wout, int kwin, int Cin, int KH, int KW, int Cout, int *splits,
+                             long long *workspace_floats);
+int bts_conv_fwd_splitk(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
+                        int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
+                        const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
+                        int act, int precision, double *stat_sum, double *stat_sumsq, int splits, float *workspace,
+                        void *stream);
 /* Tuning / bring-up switches of the narrow-output wgrad (csrc/wgrad2_tc.cu).  set_tma(0): the producers load the operands
  * from global memory (round-1 path) instead of the TMA landing ring; set_min_pixels(n): smallest map (input pixels) routed to
  * this kernel (default 12000, n < 0 restores it; tests pass 0 to reach it with small shapes). */
