@@ -126,6 +126,7 @@ SIGNATURES = {
     "bts_maxpool3s2_bwd": [_p, _ll, _p, _i, _i, _i, _i, _p, _ll, _p],
     "bts_fill_zero_f32": [_p, _ll, _p],
     "bts_input_prep": [_p, _i, _i, _p, _f, _p, _i, _i, _i, _p, _ll, _p, _p],
+    "bts_input_prep_rotated": [_p, _i, _i, _p, _f, _p, _p, _i, _i, _i, _p, _ll, _p, _p],
     "bts_eval_errors": [_p, _p, _i, _i, _f, _f, _i, _i, _i, _i, _p, _p, _p],
     "bts_depth_to_u16": [_p, _f, _ll, _p, _p],
     "bts_adamw_chunk": [],

@@ -8,7 +8,7 @@ import ctypes
 
 import torch
 
-from . import _lib
+from . import _lib, data
 
 _vp = ctypes.c_void_p
 
@@ -163,10 +163,13 @@ def silog(depth_est, depth_gt, mask, variance_focus):
 
 
 # ------------------------------------------------------------------------------------------------ data formats (SURVEY 8f)
-def input_prep(img_u8, params, out_hw, depth_u16=None, depth_div=1000.0):
+def input_prep(img_u8, params, out_hw, depth_u16=None, depth_div=1000.0, angles=None):
     """reference loader transform on the GPU (pytorch/bts_dataloader.py:128-140,202-235,244-249): img_u8 (B,Hs,Ws,3) uint8
     CUDA, params (B,9) fp32 = y0,x0,flip,augment,gamma,brightness,colour rgb -> (image (B,3,H,W) channels_last fp32,
-    depth (B,1,H,W) fp32 in metres or None)"""
+    depth (B,1,H,W) fp32 in metres or None).
+    angles: None, or B rotation angles in degrees (PIL's convention, counter-clockwise): each frame is first rotated about
+    its centre as Image.rotate(angle) does it (:122-125; bilinear image, nearest depth, 0 outside), bit for bit, and the
+    crop window is cut from the rotated frame.  The frames are the ones after the fixed crops (bts_b200.data.fixed_crop)."""
     _need_cuda(img_u8, params)
     if img_u8.dtype != torch.uint8 or img_u8.dim() != 4 or img_u8.shape[3] != 3 or not img_u8.is_contiguous():
         raise ValueError("img_u8 must be a contiguous (B,Hs,Ws,3) uint8 tensor")
@@ -182,8 +185,17 @@ def input_prep(img_u8, params, out_hw, depth_u16=None, depth_div=1000.0):
             raise ValueError("depth_u16 must be (B,Hs,Ws) uint16")
         depth_u16 = depth_u16.contiguous()
         dep = torch.empty((B, 1, H, W), device=img_u8.device, dtype=torch.float32)
-    _lib.check(_lib.lib().bts_input_prep(_ptr(img_u8), Hs, Ws, _ptr(depth_u16), float(depth_div), _ptr(params), B, H, W,
-                                         _ptr(img), 3, _ptr(dep), _stream()), "bts_input_prep")
+    if angles is None:
+        _lib.check(_lib.lib().bts_input_prep(_ptr(img_u8), Hs, Ws, _ptr(depth_u16), float(depth_div), _ptr(params), B, H, W,
+                                             _ptr(img), 3, _ptr(dep), _stream()), "bts_input_prep")
+    else:
+        angles = [float(a) for a in (angles.tolist() if torch.is_tensor(angles) else angles)]
+        if len(angles) != B:
+            raise ValueError("angles must hold one angle per sample (%d), got %d" % (B, len(angles)))
+        affine = torch.tensor([data.rotate_affine(a, Ws, Hs) for a in angles], dtype=torch.float64).to(img_u8.device)
+        _lib.check(_lib.lib().bts_input_prep_rotated(_ptr(img_u8), Hs, Ws, _ptr(depth_u16), float(depth_div), _ptr(params),
+                                                     _ptr(affine), B, H, W, _ptr(img), 3, _ptr(dep), _stream()),
+                   "bts_input_prep_rotated")
     _lib.count()
     return img, dep
 

@@ -363,6 +363,11 @@ int bts_conv_pack_weights_multi(const void *descs, int n, long long total, void 
  *   244-249), fused: uint8 HWC frames [B,Hs,Ws,3] (+ optional uint16 depth [B,Hs,Ws]) -> crop -> flip -> gamma/brightness/
  *   colour augmentation + clip -> ImageNet normalisation -> fp32 NHWC image [B,H,W,(stride)] and depth/depth_div [B,H,W].
  *   params: device float [B][9] = y0, x0, flip, augment, gamma, brightness, colour r,g,b (the random draws stay on the host).
+ * bts_input_prep_rotated: bts_input_prep after the random rotation of the whole frame (pytorch/bts_dataloader.py:122-125,
+ *   187-189): the crop window is cut from the frame as PIL's Image.rotate leaves it, bilinear for the image and nearest for
+ *   the depth, 0 outside the frame, bit-exact with Pillow.  affine: device double [B][6] = a..f of each sample's inverse
+ *   map, source point (a*(x+.5) + b*(y+.5) + c, d*(x+.5) + e*(y+.5) + f) of rotated-frame pixel (x, y), the matrix
+ *   Image.rotate passes to Image.transform (bts_b200.data.rotate_affine).  affine == NULL gives bts_input_prep's output.
  * bts_eval_errors: online-eval clamps + masks + the nine metrics of one image (pytorch/bts_main.py:144-165,275-296):
  *   metrics_out[10] = silog, abs_rel, log10, rms, sq_rel, log_rms, d1, d2, d3, n_valid; crop rows [y0,y1) cols [x0,x1);
  *   workspace = 10 doubles.
@@ -370,6 +375,9 @@ int bts_conv_pack_weights_multi(const void *descs, int n, long long total, void 
 int bts_input_prep(const unsigned char *img_u8, int Hs, int Ws, const unsigned short *depth_u16, float depth_div,
                    const float *params, int B, int H, int W, float *image_out, long long out_pixel_stride, float *depth_out,
                    void *stream);
+int bts_input_prep_rotated(const unsigned char *img_u8, int Hs, int Ws, const unsigned short *depth_u16, float depth_div,
+                           const float *params, const double *affine, int B, int H, int W, float *image_out,
+                           long long out_pixel_stride, float *depth_out, void *stream);
 int bts_eval_errors(const float *pred, const float *gt, int H, int W, float min_depth, float max_depth, int crop_y0,
                     int crop_y1, int crop_x0, int crop_x1, double *workspace, float *metrics_out, void *stream);
 int bts_depth_to_u16(const float *depth, float scale, long long n, unsigned short *out, void *stream);
