@@ -540,9 +540,13 @@ class BtsModel(nn.Module):
     def forward(self, x, focal):
         if x.is_cuda and x.dim() == 4:
             x = x.contiguous(memory_format=torch.channels_last)      # NHWC in memory for the whole path
-        from . import conv, glue
+        from . import conv, glue, graph
         if glue.no_backward(x, self):
-            # inference (bts_test.py, online eval): engine launches that leave SMs idle may run split-K
+            # inference (bts_test.py, online eval): a replayed CUDA graph when bts_b200.set_eval_graphs(True) and this
+            # input signature was seen before; otherwise eager, where engine launches that leave SMs idle may run split-K
+            out = graph.eval_forward(self, x, focal)
+            if out is not None:
+                return out
             with conv.inference():
                 return self.decoder(self.encoder(x), focal)
         return self.decoder(self.encoder(x), focal)
