@@ -64,9 +64,7 @@ _ll = ctypes.c_longlong
 SIGNATURES = {
     "bts_version": [ctypes.c_char_p, _i],
     "bts_lpg_fwd": [_p, _p, _i, _i, _i, _i, _i, _p],
-    "bts_lpg_fwd_fused": [_p, _p, _p, _p, _f, _i, _i, _i, _i, _i, _i, _p],
     "bts_lpg_bwd": [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
-    "bts_lpg_bwd_fused": [_p, _p, _p, _f, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     "bts_lpg_fwd_h": [_p, _p, _i, _i, _i, _i, _i],
     "bts_lpg_bwd_h": [_p, _p, _p, _i, _i, _i, _i, _i, _i],
     "bts_silog_fwd": [_p, _p, _p, _ll, _f, _p, _p, _p],
@@ -76,15 +74,9 @@ SIGNATURES = {
     "bts_conv_n_tile": [_i],
     "bts_conv_packed_floats": [_i, _i, _i, _i],
     "bts_conv_pack_weights": [_p, _ll, _ll, _ll, _ll, _i, _i, _i, _i, _i, _p, _p],
-    "bts_conv_fwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p],
-    "bts_conv_fwd_stats": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p, _p, _p],
-    "bts_conv_fwd_ex": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p,
-                        _p, _p],
+    "bts_conv_fwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i, _p, _p,
+                     _p, _ll, _p, _i, _i, _p, _p],
     "bts_conv_fwd_splitk_plan": [_i, _i, _i, _i, _i, _i, _i, _i, _p, _p],
-    "bts_conv_fwd_splitk": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _p, _i, _p, _ll, _i, _i,
-                            _p, _p, _i, _p, _p],
-    "bts_conv_fwd_bnbwd": [_p, _ll, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _i, _p, _i, _p, _ll, _i, _p, _ll, _p, _i,
-                           _p, _p, _p],
     "bts_bn_bwd_coef": [_p, _p, _ll, _i, _p, _p, _p, _p, _p],
     "bts_conv_group_window": [_i, _i],
     "bts_conv_packed_floats_grouped": [_i, _i, _i, _i],
@@ -100,11 +92,8 @@ SIGNATURES = {
     "bts_conv_c1_dgrad": [_p, _p, _i, _i, _i, _i, _i, _p, _ll, _ll, _ll, _p, _ll, _p],
     "bts_conv_c1_wgrad": [_p, _ll, _p, _p, _i, _i, _i, _i, _i, _p, _p, _ll, _ll, _ll, _p],
     "bts_bn_stats": [_p, _ll, _ll, _i, _p, _p, _p],
-    "bts_bn_finalize": [_p, _p, _ll, _i, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p],
-    "bts_bn_finalize_track": [_p, _p, _ll, _i, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p],
+    "bts_bn_finalize": [_p, _p, _ll, _i, _p, _p, _f, _f, _p, _p, _p, _p, _p, _p, _p, _p],
     "bts_bn_fold": [_i, _p, _p, _f, _p, _p, _p, _p, _p, _p, _p],
-    "bts_bn_relu_bwd_reduce": [_p, _ll, _p, _ll, _ll, _i, _p, _p, _p, _p, _p, _p, _p, _p],
-    "bts_bn_relu_bwd_apply": [_p, _ll, _p, _ll, _ll, _i, _p, _p, _p, _p, _ll, _i, _p],
     "bts_wgrad2_set_tma": [_i],
     "bts_wgrad2_set_min_pixels": [_ll],
     "bts_wgrad2_set_min_kblocks": [_i],

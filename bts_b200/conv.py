@@ -362,45 +362,30 @@ def conv2d_tc(x, weight, stride=1, padding=0, dilation=1, pre_scale=None, pre_sh
             nsplit, wsf = splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Co, 0 if splits is None else int(splits))
         if nsplit > 1:
             ws = torch.empty(wsf, device=x.device, dtype=torch.float32)
+    xb = st = None
+    xbs = relu = 0
     if bn_bwd is not None:
         xb, st, relu = bn_bwd
         xb, xbs = _nhwc_view(xb)
         if stats is None or act is not None or pre_scale is not None or pre_relu or tuple(xb.shape) != (B, Co, Hout, Wout) \
                 or tuple(st.shape) != (4, Co) or not st.is_contiguous():
             raise ValueError("bn_bwd needs zeroed stats, no act / pre-op, x_bn shaped like the output and st = [4, Cout]")
-        with torch.cuda.device(x.device):
-            rc = _traced("dgrad" if transpose_flip else "fwd",
-                         "%dx%dx%d %d->%d k%d d%d s%d%s bnb" % (B, Hs, Ws, Cin, Co, KH, dilation, stride, " zs" if mode == 2 else ""),
-                         lambda: _lib.lib().bts_conv_fwd_bnbwd(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
-                                                               Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding,
-                                                               dilation, _ptr(packed), Co, _ptr(out), os_, int(precision),
-                                                               _ptr(xb), xbs, _ptr(st), int(bool(relu)), _ptr(stats[0]),
-                                                               _ptr(stats[1]), _stream()),
-                         2.0 * B * Hout * Wout * Co * (Cin // groups) * KH * KW)
-        _lib.check(rc, "bts_conv_fwd_bnbwd")
-        _lib.count()
-        return out
     st0 = _ptr(stats[0]) if stats is not None else None
     st1 = _ptr(stats[1]) if stats is not None else None
     with torch.cuda.device(x.device):
-        if ws is not None:
-            call = lambda: _lib.lib().bts_conv_fwd_splitk(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
-                                                          Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding,
-                                                          dilation, _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift),
-                                                          int(pre_relu), _ptr(out), os_, ACT[act], int(precision), st0, st1,
-                                                          nsplit, _ptr(ws), _stream())
-        else:
-            call = lambda: _lib.lib().bts_conv_fwd_ex(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
-                                                      Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding, dilation,
-                                                      _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift), int(pre_relu),
-                                                      _ptr(out), os_, ACT[act], int(precision), st0, st1, _stream())
         rc = _traced("dgrad" if transpose_flip else "fwd",
-                     "%dx%dx%d %d->%d k%d d%d s%d%s%s%s" % (B, Hs, Ws, Cin, Co, KH, dilation, stride,
-                                                           " up" if upsample2 else (" zs" if mode == 2 else ""),
-                                                           " g%d" % groups if groups > 1 else "",
-                                                           " sk%d" % nsplit if ws is not None else ""),
-                     call, 2.0 * B * Hout * Wout * Co * (Cin // groups) * KH * KW / (4.0 if mode == 2 else 1.0))
-    _lib.check(rc, "bts_conv_fwd_splitk" if ws is not None else "bts_conv_fwd_ex")
+                     "%dx%dx%d %d->%d k%d d%d s%d%s%s%s%s" % (B, Hs, Ws, Cin, Co, KH, dilation, stride,
+                                                             " up" if upsample2 else (" zs" if mode == 2 else ""),
+                                                             " g%d" % groups if groups > 1 else "",
+                                                             " sk%d" % nsplit if ws is not None else "",
+                                                             " bnb" if bn_bwd is not None else ""),
+                     lambda: _lib.lib().bts_conv_fwd(_ptr(x), xs, B, Hs, Ws, mode, Hout if mode == 2 else 0,
+                                                     Wout if mode == 2 else 0, kwin, Cin, KH, KW, stride, padding, dilation,
+                                                     _ptr(packed), Co, _ptr(pre_scale), _ptr(pre_shift), int(pre_relu),
+                                                     _ptr(out), os_, ACT[act], int(precision), st0, st1, _ptr(xb), xbs,
+                                                     _ptr(st), int(bool(relu)), nsplit, _ptr(ws), _stream()),
+                     2.0 * B * Hout * Wout * Co * (Cin // groups) * KH * KW / (4.0 if mode == 2 else 1.0))
+    _lib.check(rc, "bts_conv_fwd")
     _lib.count(2 if ws is not None else 1)
     return out
 

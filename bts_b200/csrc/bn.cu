@@ -6,10 +6,11 @@
 // What remains are per-channel reductions over the NHWC activation (channel = fastest index -> lanes own channels,
 // fully coalesced) and one elementwise backward pass:
 //   bts_bn_stats      : sum, sum of squares per channel (fp32 per-thread strips, fp64 cross-block accumulation)
-//   bts_bn_finalize   : mean / biased var -> scale, shift, invstd; running-stat update with momentum (unbiased var)
-//   bts_bn_relu_bwd_reduce : S1 = sum g*[y>0], S2 = sum g*[y>0]*xhat            (y = x*scale+shift, xhat = (x-mean)*invstd)
-//   bts_bn_relu_bwd_apply  : dx = scale * ( g*[y>0] - S1/N - xhat*S2/N ), written or ACCUMULATED into a (slice of a)
-//                            gradient slab -- the concat fan-out of a dense block sums into one buffer, no add kernels.
+//   bts_bn_finalize   : mean / biased var -> scale, shift, invstd; running-stat update with momentum (unbiased var),
+//                       num_batches_tracked += 1
+//   bts_bn_bwd_reduce : S1 = sum g*mask, S2 = sum g*mask*xhat      (y = x*scale+shift, xhat = (x-mean)*invstd, mask of `act`)
+//   bts_bn_bwd_apply  : dx = scale * ( g*mask - S1/N - xhat*S2/N ), written or ACCUMULATED into a (slice of a)
+//                       gradient slab -- the concat fan-out of a dense block sums into one buffer, no add kernels.
 // All tensors are NHWC with an explicit pixel stride, so channel slices of wider slabs work in place.
 #include "common.cuh"
 
@@ -342,20 +343,8 @@ extern "C" int bts_bn_stats(const float *x, long long x_pixel_stride, long long 
 
 extern "C" int bts_bn_finalize(const double *sum, const double *sumsq, long long N, int C, const float *gamma,
                                const float *beta, float eps, float momentum, float *running_mean, float *running_var,
-                               float *scale, float *shift, float *mean, float *invstd, void *stream) {
-    if (!sum || !sumsq || !scale || !shift || !mean || !invstd || N < 1 || C < 1) return BTS_EINVAL;
-    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(sum, sumsq, N, C, gamma, beta, eps, momentum,
-                                                                          running_mean, running_var, scale, shift, mean, invstd,
-                                                                          nullptr);
-    BTS_LAUNCH_CHECK();
-    return 0;
-}
-
-// the same, also incrementing the module's int64 `num_batches_tracked` buffer in the same launch
-extern "C" int bts_bn_finalize_track(const double *sum, const double *sumsq, long long N, int C, const float *gamma,
-                                     const float *beta, float eps, float momentum, float *running_mean, float *running_var,
-                                     long long *num_batches_tracked, float *scale, float *shift, float *mean, float *invstd,
-                                     void *stream) {
+                               long long *num_batches_tracked, float *scale, float *shift, float *mean, float *invstd,
+                               void *stream) {
     if (!sum || !sumsq || !scale || !shift || !mean || !invstd || N < 1 || C < 1) return BTS_EINVAL;
     bn_finalize_kernel<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(sum, sumsq, N, C, gamma, beta, eps, momentum,
                                                                           running_mean, running_var, scale, shift, mean, invstd,
@@ -441,19 +430,13 @@ extern "C" int bts_bn_bwd_correct(const float *x, long long x_pixel_stride, long
 }
 
 // (k0, k1) coefficients of the backward apply pass from already-reduced sums (the reduction fused into a dgrad epilogue,
-// bts_conv_fwd_bnbwd)
+// bts_conv_fwd with x_bn / bn_st)
 extern "C" int bts_bn_bwd_coef(const double *S1, const double *S2, long long M, int C, const float *scale, const float *mean,
                                const float *invstd, float *coef, void *stream) {
     if (!S1 || !S2 || !scale || !mean || !invstd || !coef || M < 1 || C < 1) return BTS_EINVAL;
     bn_bwd_coef_kernel<<<(C + 127) / 128, 128, 0, (cudaStream_t)stream>>>(S1, S2, M, C, scale, mean, invstd, coef);
     BTS_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int bts_bn_relu_bwd_reduce(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
-                                      long long M, int C, const float *scale, const float *shift, const float *mean,
-                                      const float *invstd, double *S1, double *S2, float *coef, void *stream) {
-    return bts_bn_bwd_reduce(x, x_pixel_stride, g, g_pixel_stride, M, C, scale, shift, mean, invstd, 1, S1, S2, coef, stream);
 }
 
 extern "C" int bts_bn_bwd_apply(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
@@ -469,11 +452,4 @@ extern "C" int bts_bn_bwd_apply(const float *x, long long x_pixel_stride, const 
                                                                           act);
     BTS_LAUNCH_CHECK();
     return 0;
-}
-
-extern "C" int bts_bn_relu_bwd_apply(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
-                                     long long M, int C, const float *scale, const float *shift, const float *coef,
-                                     float *out, long long out_pixel_stride, int accumulate, void *stream) {
-    return bts_bn_bwd_apply(x, x_pixel_stride, g, g_pixel_stride, M, C, scale, shift, coef, 1, out, out_pixel_stride,
-                            accumulate, stream);
 }

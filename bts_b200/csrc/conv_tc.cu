@@ -91,7 +91,7 @@ struct ConvParams {
     tc::FastDiv fd_cq, fd_kw;
     double *stat_sum, *stat_sumsq;   // optional per-output-channel sum / sum of squares of the (activated) output
     // BatchNorm-backward reduction fused into a dgrad's epilogue (bnb_x != null): the tile being written is g = dL/d relu(bn(x));
-    // stat_sum[c] += sum_p g*[bn(x)>0],  stat_sumsq[c] += sum_p g*[bn(x)>0]*xhat   (bts_bn_relu_bwd_reduce without its pass)
+    // stat_sum[c] += sum_p g*[bn(x)>0],  stat_sumsq[c] += sum_p g*[bn(x)>0]*xhat   (bts_bn_bwd_reduce without its pass)
     const float *bnb_x; long long bnb_xs;
     const float *bnb_st;             // [4][Cout]: scale, shift, mean, invstd
     int bnb_relu;
@@ -760,7 +760,7 @@ extern "C" int bts_conv_pack_weights(const float *w, long long s_co, long long s
 // Grouped convolution whose groups tile a 128-wide diagonal block (ResNeXt 3x3: width % kwin == 0, kwin % cpg == 0):
 // w is (width, cpg, KH, KW); the packed operator has width/n_tile n-tiles of n_tile = bts_conv_group_n_tile(kwin) rows,
 // each over the K window of kwin channels that holds its rows -- zeros outside the row's group.  Run with
-// bts_conv_fwd_ex(kwin = bts_conv_group_window(width, cpg)).
+// bts_conv_fwd(kwin = bts_conv_group_window(width, cpg)).
 extern "C" int bts_conv_group_window(int width, int cpg) {
     if (width < 1 || cpg < 1 || width % cpg) return 0;
     int k = 128;
@@ -808,33 +808,37 @@ extern "C" int bts_conv_pack_weights_grouped(const float *w, long long s_co, lon
     return 0;
 }
 
-struct BnBwdArgs {
-    const float *x; long long xs; const float *st; int relu;
-};
-
-static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int out_h,
-                         int out_w, int kwin, int Cin,
-                         int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                         const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
-                         long long out_pixel_stride, int act, int precision, double *stat_sum, double *stat_sumsq,
-                         void *stream, const BnBwdArgs *bnb = nullptr, int splits = 1, float *workspace = nullptr) {
+// Forward / dgrad entry point (see bts_b200.h).  Split mode (workspace != NULL): the conv kernel writes raw partial tile
+// sums into `workspace` ([splits][M][Cpad]), conv_splitk_reduce_kernel adds them and applies the activation into out.
+// Every check of an argument combination comes before the first CUDA runtime call (bts_num_sms).
+extern "C" int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h,
+                            int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack,
+                            int Cout, const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
+                            long long out_pixel_stride, int act, int precision, double *stat_sum, double *stat_sumsq,
+                            const float *x_bn, long long x_bn_stride, const float *bn_st, int relu, int splits,
+                            float *workspace, void *stream) {
     if (!x || !wpack || !out || B < 0 || Hs < 1 || Ws < 1 || Cin < 1 || Cout < 1 || KH < 1 || KW < 1 || stride < 1 ||
         pad < 0 || dil < 1)
         return BTS_EINVAL;
     if ((pre_scale == nullptr) != (pre_shift == nullptr)) return BTS_EINVAL;
     if (pre_scale && Cin > MAX_CIN_SMEM) return BTS_EINVAL;
     if (act < 0 || act > 2 || precision < 0 || precision > 1) return BTS_EINVAL;
-    if (upsample2 < 0 || upsample2 > 2 || kwin < 0) return BTS_EINVAL;
-    if (upsample2 == 2 && (stride != 1 || out_h < 1 || out_w < 1)) return BTS_EINVAL;
+    if (source_mode < 0 || source_mode > 2 || kwin < 0) return BTS_EINVAL;
+    if (source_mode == 2 && (stride != 1 || out_h < 1 || out_w < 1)) return BTS_EINVAL;
     if (kwin && (pre_scale || Cin % kwin || Cout % kwin)) return BTS_EINVAL;   // whole windows; no pre-op on grouped convs
     if (!bts_aligned16(wpack)) return BTS_EALIGN;
+    if ((stat_sum == nullptr) != (stat_sumsq == nullptr)) return BTS_EINVAL;
+    if (stat_sum && act != 0) return BTS_EINVAL;                        // statistics of the raw conv output only
+    const bool bnb = x_bn || bn_st;
+    if (bnb && (!x_bn || !bn_st || !stat_sum)) return BTS_EINVAL;       // its sums go to stat_sum / stat_sumsq
+    if (splits < 1 || (splits > 1 && !workspace)) return BTS_EINVAL;
     const bool split_mode = workspace != nullptr;
-    if (split_mode && (splits < 1 || stat_sum || stat_sumsq || bnb)) return BTS_EINVAL;   // raw sums: no epilogue reductions
+    if (split_mode && (stat_sum || bnb)) return BTS_EINVAL;             // raw sums: no epilogue reductions
     if (split_mode && !bts_aligned16(workspace)) return BTS_EALIGN;
     if (B == 0) return 0;
     if ((long long)B * Hs * Ws * x_pixel_stride >= 0x7fffffffLL) return BTS_EINVAL;   // 32-bit element offsets
     ConvParams p;
-    p.x = x; p.xs = x_pixel_stride; p.B = B; p.Hs = Hs; p.Ws = Ws; p.up = upsample2; p.Cin = kwin ? kwin : Cin;
+    p.x = x; p.xs = x_pixel_stride; p.B = B; p.Hs = Hs; p.Ws = Ws; p.up = source_mode; p.Cin = kwin ? kwin : Cin;
     p.kwin = kwin;
     p.KH = KH; p.KW = KW; p.stride = stride; p.pad = pad; p.dil = dil;
     p.wpack = wpack; p.Cout = Cout;
@@ -844,13 +848,7 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     p.pre_scale = pre_scale; p.pre_shift = pre_shift; p.pre_relu = pre_relu ? 1 : 0;
     p.out = out; p.os = out_pixel_stride; p.act = act;
     p.stat_sum = stat_sum; p.stat_sumsq = stat_sumsq;
-    if ((stat_sum == nullptr) != (stat_sumsq == nullptr)) return BTS_EINVAL;
-    p.bnb_x = nullptr; p.bnb_xs = 0; p.bnb_st = nullptr; p.bnb_relu = 0;
-    if (bnb) {
-        if (!bnb->x || !bnb->st || !stat_sum || act != 0) return BTS_EINVAL;
-        p.bnb_x = bnb->x; p.bnb_xs = bnb->xs; p.bnb_st = bnb->st; p.bnb_relu = bnb->relu ? 1 : 0;
-    }
-    if (stat_sum && act != 0) return BTS_EINVAL;                        // statistics of the raw conv output only
+    p.bnb_x = x_bn; p.bnb_xs = x_bn_stride; p.bnb_st = bn_st; p.bnb_relu = relu ? 1 : 0;
     const int Hin = p.up ? 2 * Hs : Hs, Win = p.up ? 2 * Ws : Ws;
     p.Hv = Hin; p.Wv = Win;      // mode 2: live source coordinates are the even ones below 2Hs x 2Ws, zeros everywhere else
     p.Hout = p.up == 2 ? out_h : (Hin + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
@@ -946,42 +944,6 @@ static int conv_fwd_impl(const float *x, long long x_pixel_stride, int B, int Hs
     return 0;
 }
 
-extern "C" int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
-                            int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                            const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
-                            long long out_pixel_stride, int act, int precision, void *stream) {
-    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, upsample2 ? 1 : 0, 0, 0, 0, Cin, KH, KW, stride, pad, dil, wpack, Cout,
-                         pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, nullptr, nullptr, stream);
-}
-
-extern "C" int bts_conv_fwd_stats(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
-                                  int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                                  const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
-                                  long long out_pixel_stride, int act, int precision, double *stat_sum,
-                                  double *stat_sumsq, void *stream) {
-    if (!stat_sum || !stat_sumsq) return BTS_EINVAL;
-    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, upsample2 ? 1 : 0, 0, 0, 0, Cin, KH, KW, stride, pad, dil, wpack, Cout,
-                         pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq, stream);
-}
-
-// General entry point: everything bts_conv_fwd does, plus
-//   source_mode 2: the source is the zero-stuffed x2 expansion of x (value at (2i,2j) = x[i,j], zeros elsewhere) and the
-//       output has the given out_h x out_w -- with the transposed, tap-flipped packed operator and pad' = dil*(K-1) - pad
-//       this is the input gradient of a STRIDE-2 convolution whose input was out_h x out_w (ResNet / ResNeXt stages,
-//       pytorch/bts.py:282-296 via torchvision); call with stride = 1;
-//   kwin > 0: block-diagonal ("grouped") operator: output channels [nt*kwin, (nt+1)*kwin) only see input channels
-//       [nt*kwin, (nt+1)*kwin) (ResNeXt 3x3 convs, 32 groups: groups are packed kwin/cpg to a 128-wide diagonal block,
-//       see bts_conv_pack_weights_grouped); Cin and Cout are the layer's total channel counts.
-extern "C" int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h,
-                               int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
-                               const float *wpack, int Cout, const float *pre_scale, const float *pre_shift, int pre_relu,
-                               float *out, long long out_pixel_stride, int act, int precision, double *stat_sum,
-                               double *stat_sumsq, void *stream) {
-    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
-                         Cout, pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq,
-                         stream);
-}
-
 // Split-K plan of a forward / dgrad launch (see bts_b200.h).  A launch splits only when its tiles fill at most half the SMs:
 // splits = as many as keep tiles * splits within one wave of bts_num_sms() and every split at least SPLITK_MIN_KB k-blocks
 // long (its padded tail included), so that each tile of a split streams more k-blocks than the deepest stage ring holds
@@ -1021,19 +983,6 @@ extern "C" int bts_conv_fwd_splitk_plan(int B, int Hout, int Wout, int kwin, int
     return 0;
 }
 
-// bts_conv_fwd_ex in split-K mode (see bts_b200.h): the conv kernel writes raw partial tile sums into `workspace`
-// ([splits][M][Cpad]), conv_splitk_reduce_kernel adds them and applies the activation into out.
-extern "C" int bts_conv_fwd_splitk(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h,
-                                   int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
-                                   const float *wpack, int Cout, const float *pre_scale, const float *pre_shift, int pre_relu,
-                                   float *out, long long out_pixel_stride, int act, int precision, double *stat_sum,
-                                   double *stat_sumsq, int splits, float *workspace, void *stream) {
-    if (!workspace) return BTS_EINVAL;
-    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
-                         Cout, pre_scale, pre_shift, pre_relu, out, out_pixel_stride, act, precision, stat_sum, stat_sumsq,
-                         stream, nullptr, splits, workspace);
-}
-
 // descs: device array of n PackDesc (layout above; built by the host side once per model), total = sum of packed_floats / 2
 extern "C" int bts_conv_pack_weights_multi(const void *descs, int n, long long total, void *stream) {
     if (!descs || n < 1 || total < 1) return BTS_EINVAL;
@@ -1043,19 +992,4 @@ extern "C" int bts_conv_pack_weights_multi(const void *descs, int n, long long t
     pack_weights_multi_kernel<<<(int)grid, 256, 0, (cudaStream_t)stream>>>(reinterpret_cast<const PackDesc *>(descs), n, total);
     BTS_LAUNCH_CHECK();
     return 0;
-}
-
-// dgrad whose epilogue also reduces the BatchNorm(+ReLU) backward sums of the layer in front of the conv: the tile written
-// is g = dL/d[relu](bn(x_bn)); S1[c] += sum_p g*mask, S2[c] += sum_p g*mask*xhat with mask = [bn(x)>0] (relu) or 1,
-// xhat = (x - mean)*invstd.  x_bn: the BatchNorm INPUT at the output's pixels/channels (NHWC, pixel stride x_bn_stride),
-// bn_st: [4][Cout] = scale, shift, mean, invstd (bts_bn_finalize layout).  S1/S2 must be zeroed.  Replaces the separate
-// bts_bn_relu_bwd_reduce pass over (x, g) -- 174 launches and two full tensor reads per DenseNet-161 step.
-extern "C" int bts_conv_fwd_bnbwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h,
-                                  int out_w, int kwin, int Cin, int KH, int KW, int stride, int pad, int dil,
-                                  const float *wpack, int Cout, float *out, long long out_pixel_stride, int precision,
-                                  const float *x_bn, long long x_bn_stride, const float *bn_st, int relu, double *S1,
-                                  double *S2, void *stream) {
-    BnBwdArgs a{x_bn, x_bn_stride, bn_st, relu};
-    return conv_fwd_impl(x, x_pixel_stride, B, Hs, Ws, source_mode, out_h, out_w, kwin, Cin, KH, KW, stride, pad, dil, wpack,
-                         Cout, nullptr, nullptr, 0, out, out_pixel_stride, 0, precision, S1, S2, stream, &a);
 }

@@ -402,49 +402,28 @@ int check_common(const void *plane, int B, int h, int w, int r, int layout) {
 
 }  // namespace
 
-extern "C" int bts_lpg_fwd_fused(const float *plane, float *depth, float *scaled, float *ds, float max_depth,
-                                 int ds_stride, int B, int h, int w, int r, int layout, void *stream) {
-    int rc = check_common(plane, B, h, w, r, layout);
-    if (rc) return rc;
-    if ((long long)B * h * w == 0) return 0;   // empty input: nothing to do (TF op allocates an empty output)
-    if (!depth && !scaled && !ds) return BTS_EINVAL;
-    if ((scaled || ds) && !(max_depth > 0.f)) return BTS_EINVAL;
-    if (ds && (ds_stride < 1 || (h * r) % ds_stride || (w * r) % ds_stride)) return BTS_EINVAL;
-    if ((long long)B * h * w == 0) return 0;   // empty input: nothing to do (TF op allocates an empty output)
-    cudaStream_t st = (cudaStream_t)stream;
-    const int S = ds ? ds_stride : 1;
-    const PlaneSrc src{plane, nullptr, 0.f};
-    return layout == BTS_LAYOUT_NCHW ? launch_fwd<BTS_LAYOUT_NCHW>(src, depth, scaled, ds, max_depth, S, B, h, w, r, st)
-                                     : launch_fwd<BTS_LAYOUT_NHWC>(src, depth, scaled, ds, max_depth, S, B, h, w, r, st);
-}
-
 extern "C" int bts_lpg_fwd(const float *plane, float *depth, int B, int h, int w, int r, int layout, void *stream) {
-    if (!depth && (long long)B * h * w != 0) return BTS_EINVAL;
-    return bts_lpg_fwd_fused(plane, depth, nullptr, nullptr, 1.f, 1, B, h, w, r, layout, stream);
-}
-
-extern "C" int bts_lpg_bwd_fused(const float *d_depth, const float *d_scaled, const float *d_ds, float max_depth,
-                                 int ds_stride, const float *plane, float *dplane, int B, int h, int w, int r,
-                                 int layout, int tf_compat, void *stream) {
     int rc = check_common(plane, B, h, w, r, layout);
     if (rc) return rc;
-    if ((long long)B * h * w == 0) return 0;
-    if (!dplane || (!d_depth && !d_scaled && !d_ds)) return BTS_EINVAL;
-    if ((d_scaled || d_ds) && !(max_depth > 0.f)) return BTS_EINVAL;
-    if (d_ds && (ds_stride < 1 || (h * r) % ds_stride || (w * r) % ds_stride)) return BTS_EINVAL;
-    if ((long long)B * h * w == 0) return 0;
+    if ((long long)B * h * w == 0) return 0;   // empty input: nothing to do (TF op allocates an empty output)
+    if (!depth) return BTS_EINVAL;
     cudaStream_t st = (cudaStream_t)stream;
-    const int S = d_ds ? ds_stride : 1;
     const PlaneSrc src{plane, nullptr, 0.f};
-    return layout == BTS_LAYOUT_NCHW
-               ? launch_bwd<BTS_LAYOUT_NCHW>(d_depth, d_scaled, d_ds, max_depth, S, src, dplane, B, h, w, r, tf_compat, st)
-               : launch_bwd<BTS_LAYOUT_NHWC>(d_depth, d_scaled, d_ds, max_depth, S, src, dplane, B, h, w, r, tf_compat, st);
+    return layout == BTS_LAYOUT_NCHW ? launch_fwd<BTS_LAYOUT_NCHW>(src, depth, nullptr, nullptr, 1.f, 1, B, h, w, r, st)
+                                     : launch_fwd<BTS_LAYOUT_NHWC>(src, depth, nullptr, nullptr, 1.f, 1, B, h, w, r, st);
 }
 
 extern "C" int bts_lpg_bwd(const float *dy, const float *plane, float *dplane, int B, int h, int w, int r, int layout,
                            int tf_compat, void *stream) {
-    if (!dy && (long long)B * h * w != 0) return BTS_EINVAL;
-    return bts_lpg_bwd_fused(dy, nullptr, nullptr, 1.f, 1, plane, dplane, B, h, w, r, layout, tf_compat, stream);
+    int rc = check_common(plane, B, h, w, r, layout);
+    if (rc) return rc;
+    if ((long long)B * h * w == 0) return 0;
+    if (!dy || !dplane) return BTS_EINVAL;
+    cudaStream_t st = (cudaStream_t)stream;
+    const PlaneSrc src{plane, nullptr, 0.f};
+    return layout == BTS_LAYOUT_NCHW
+               ? launch_bwd<BTS_LAYOUT_NCHW>(dy, nullptr, nullptr, 1.f, 1, src, dplane, B, h, w, r, tf_compat, st)
+               : launch_bwd<BTS_LAYOUT_NHWC>(dy, nullptr, nullptr, 1.f, 1, src, dplane, B, h, w, r, tf_compat, st);
 }
 
 // ---- fused plane-coefficient head tail + LPG (pytorch/bts.py:112-120 + 223-229) -------------------

@@ -15,12 +15,11 @@ kernels and two cuDNN convs forward, and the mirror image plus one `add` per con
 Parameters and buffers stay the torchvision modules' own (names, shapes, running-stat semantics: momentum, unbiased
 running variance, num_batches_tracked), so checkpoints and bts_main.set_misc's name-based freezing are unaffected.
 """
-import ctypes
 import os
 
 import torch
 
-from . import _lib, conv
+from . import _lib, conv, glue
 from .ops import _ptr, _stream
 
 EPI_STATS = True   # BatchNorm batch statistics reduced in the producing conv's epilogue (csrc/conv_tc.cu)
@@ -31,59 +30,6 @@ def _view(t):
     if t2 is not t:
         raise ValueError("fused BN ops need NHWC-in-memory tensors")
     return t, s
-
-
-def bn_stats(x):
-    """per-channel (sum, sum of squares) of an NHWC tensor / channel slice -> two fp64 vectors"""
-    x, xs = _view(x)
-    B, C, H, W = x.shape
-    out = torch.empty((2, C), device=x.device, dtype=torch.float64)
-    _lib.check(_lib.lib().bts_bn_stats(_ptr(x), xs, B * H * W, C, _ptr(out[0]), _ptr(out[1]), _stream()), "bts_bn_stats")
-    _lib.count()
-    return out
-
-
-def bn_finalize(sums, n, bn, training):
-    """(scale, shift, mean, invstd) [4,C] for BatchNorm module `bn`; updates its running statistics like nn.BatchNorm2d"""
-    C = bn.num_features
-    out = torch.empty((4, C), device=bn.running_mean.device, dtype=torch.float32)
-    L = _lib.lib()
-    g = bn.weight.detach() if bn.weight is not None else None
-    b = bn.bias.detach() if bn.bias is not None else None
-    if training:
-        track = bn.track_running_stats and bn.running_mean is not None
-        mom = bn.momentum if bn.momentum is not None else 0.1
-        if sums.shape[1] != C:
-            raise ValueError("statistics cover %d channels, BatchNorm has %d" % (sums.shape[1], C))
-        nbt = bn.num_batches_tracked if (track and bn.num_batches_tracked is not None) else None
-        _lib.check(L.bts_bn_finalize_track(_ptr(sums[0]), _ptr(sums[1]), n, C, _ptr(g), _ptr(b), float(bn.eps), float(mom),
-                                           _ptr(bn.running_mean) if track else None, _ptr(bn.running_var) if track else None,
-                                           _ptr(nbt), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), _stream()),
-                   "bts_bn_finalize_track")
-    else:
-        _lib.check(L.bts_bn_fold(C, _ptr(g), _ptr(b), float(bn.eps), _ptr(bn.running_mean), _ptr(bn.running_var),
-                                 _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), _stream()), "bts_bn_fold")
-    _lib.count()
-    return out
-
-
-def bn_relu_backward(x, g, st, use_stats, out, accumulate):
-    """out (=|+=) d/dx of relu(bn(x)) given g = d/d(relu out); returns (S1, S2) = (dbeta, dgamma) as fp64 [2,C]"""
-    x, xs = _view(x)
-    g, gs = _view(g)
-    out, os_ = _view(out)
-    B, C, H, W = x.shape
-    M = B * H * W
-    L = _lib.lib()
-    S = torch.empty((2, C), device=x.device, dtype=torch.float64)
-    coef = torch.empty((2, C), device=x.device, dtype=torch.float32)
-    _lib.check(L.bts_bn_relu_bwd_reduce(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]), _ptr(st[2]), _ptr(st[3]),
-                                        _ptr(S[0]), _ptr(S[1]), _ptr(coef), _stream()), "bts_bn_relu_bwd_reduce")
-    _lib.check(L.bts_bn_relu_bwd_apply(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]),
-                                       _ptr(coef) if use_stats else None, _ptr(out), os_, int(accumulate), _stream()),
-               "bts_bn_relu_bwd_apply")
-    _lib.count(3)
-    return S
 
 
 # One-pass norm1 backward of a dense layer: the sums-independent part of dx is accumulated into the gradient slab by the
@@ -118,14 +64,15 @@ def bn_backward_correct(x, K, out):
     _lib.count()
 
 
-# BatchNorm-backward sums reduced in the dgrad epilogue (bts_conv_fwd_bnbwd) instead of a separate pass.  The epilogue
-# already paces the short-K dgrads, and the fused form adds strided reads of x and of the per-channel parameters to it, so
-# the separate streaming reduce pass is the default; the fused form stays available (and tested) for long-K layers.
+# BatchNorm-backward sums reduced in the dgrad epilogue (bts_conv_fwd with x_bn / bn_st) instead of a separate pass.  The
+# epilogue already paces the short-K dgrads, and the fused form adds strided reads of x and of the per-channel parameters
+# to it, so the separate streaming reduce pass is the default; the fused form stays available (and tested) for long-K
+# layers.
 EPI_BNBWD = os.environ.get("BTS_B200_EPI_BNBWD", "0") == "1"
 
 
 def bn_relu_backward_from_sums(x, g, st, S, use_stats, out, accumulate):
-    """the apply half of bn_relu_backward when S = (S1, S2) already came out of the dgrad epilogue"""
+    """the apply half of glue.bn_backward(act=1) when S = (S1, S2) already came out of the dgrad epilogue"""
     x, xs = _view(x)
     g, gs = _view(g)
     out, os_ = _view(out)
@@ -137,8 +84,8 @@ def bn_relu_backward_from_sums(x, g, st, S, use_stats, out, accumulate):
         coef = torch.empty((2, C), device=x.device, dtype=torch.float32)
         _lib.check(L.bts_bn_bwd_coef(_ptr(S[0]), _ptr(S[1]), M, C, _ptr(st[0]), _ptr(st[2]), _ptr(st[3]), _ptr(coef), _stream()),
                    "bts_bn_bwd_coef")
-    _lib.check(L.bts_bn_relu_bwd_apply(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]), _ptr(coef), _ptr(out), os_,
-                                       int(accumulate), _stream()), "bts_bn_relu_bwd_apply")
+    _lib.check(L.bts_bn_bwd_apply(_ptr(x), xs, _ptr(g), gs, M, C, _ptr(st[0]), _ptr(st[1]), _ptr(coef), 1, _ptr(out), os_,
+                                  int(accumulate), _stream()), "bts_bn_bwd_apply")
     _lib.count(2)
     return S
 
@@ -169,7 +116,7 @@ class _DenseBlockFn(torch.autograd.Function):
         slab[:, :C0].copy_(x)
         sums = torch.empty((2, Ct), device=x.device, dtype=torch.float64)
         if training:
-            sums[:, :C0] = bn_stats(slab[:, :C0])
+            sums[:, :C0] = glue.bn_stats(slab[:, :C0])
         saved_b, saved_st = [], []
         C = C0
         # the zeroed [2, C] accumulators of the epilogue statistics of every layer, carved out of ONE zero fill
@@ -184,17 +131,19 @@ class _DenseBlockFn(torch.autograd.Function):
 
         for li, layer in enumerate(layers):
             w1, w2 = params[6 * li + 2], params[6 * li + 5]
-            st1 = bn_finalize(sums[:, :C] if training else None, n, layer.norm1, training)
+            bn1, bn2 = layer.norm1, layer.norm2
+            st1 = glue.bn_finalize(sums[:, :C] if training else None, n, bn1, bn1.weight, bn1.bias, training)
             epi = training and EPI_STATS and w1.shape[0] <= 256 and growth <= 256
             sb = zeros2(w1.shape[0]) if epi else None
             b = conv.conv2d_tc(slab[:, :C], w1, 1, 0, 1, pre_scale=st1[0], pre_shift=st1[1], pre_relu=True, stats=sb)
-            st2 = bn_finalize((sb if epi else bn_stats(b)) if training else None, n, layer.norm2, training)
+            st2 = glue.bn_finalize((sb if epi else glue.bn_stats(b)) if training else None, n, bn2, bn2.weight, bn2.bias,
+                                   training)
             more = training and li + 1 < len(layers)
             sn = zeros2(growth) if (epi and more) else None
             conv.conv2d_tc(b, w2, 1, 1, 1, pre_scale=st2[0], pre_shift=st2[1], pre_relu=True, out=slab[:, C:C + growth],
                            stats=sn)
             if more:
-                sums[:, C:C + growth] = sn if sn is not None else bn_stats(slab[:, C:C + growth])
+                sums[:, C:C + growth] = sn if sn is not None else glue.bn_stats(slab[:, C:C + growth])
             saved_b.append(b)
             saved_st += [st1, st2]
             C += growth
@@ -234,7 +183,7 @@ class _DenseBlockFn(torch.autograd.Function):
             else:
                 g_a2 = conv.conv2d_tc(g_out, w2, 1, 1, 1, transpose_flip=True)
                 # ---- norm2 + relu2 backward (in place on g_a2)
-                S = bn_relu_backward(b, g_a2, st2, training, g_a2, False)
+                _, S = glue.bn_backward(b, g_a2, st2, training, 1, out=g_a2)
             if need[6 * li + 3]:
                 grads[6 * li + 3] = S[1].float()
             if need[6 * li + 4]:
@@ -252,7 +201,7 @@ class _DenseBlockFn(torch.autograd.Function):
                 if onepass:
                     S = bn_relu_backward_onepass(xin, g_a1, st1, G[:, :C], K)
                 else:
-                    S = bn_relu_backward(xin, g_a1, st1, training, G[:, :C], True)
+                    _, S = glue.bn_backward(xin, g_a1, st1, training, 1, out=G[:, :C], accumulate=True)
             if need[6 * li + 0]:
                 grads[6 * li + 0] = S[1].float()
             if need[6 * li + 1]:

@@ -65,11 +65,13 @@ def bn_finalize(sums, n, bn, gamma, beta, training):
     if training:
         track = bn.track_running_stats and bn.running_mean is not None
         mom = bn.momentum if bn.momentum is not None else 0.1
+        if sums.shape[1] != C:
+            raise ValueError("statistics cover %d channels, BatchNorm has %d" % (sums.shape[1], C))
         nbt = bn.num_batches_tracked if (track and bn.num_batches_tracked is not None) else None
-        _lib.check(L.bts_bn_finalize_track(_ptr(sums[0]), _ptr(sums[1]), n, C, _ptr(g), _ptr(b), float(bn.eps), float(mom),
-                                           _ptr(bn.running_mean) if track else None, _ptr(bn.running_var) if track else None,
-                                           _ptr(nbt), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), _stream()),
-                   "bts_bn_finalize_track")
+        _lib.check(L.bts_bn_finalize(_ptr(sums[0]), _ptr(sums[1]), n, C, _ptr(g), _ptr(b), float(bn.eps), float(mom),
+                                     _ptr(bn.running_mean) if track else None, _ptr(bn.running_var) if track else None,
+                                     _ptr(nbt), _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), _stream()),
+                   "bts_bn_finalize")
     else:
         _lib.check(L.bts_bn_fold(C, _ptr(g), _ptr(b), float(bn.eps), _ptr(bn.running_mean), _ptr(bn.running_var),
                                  _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), _ptr(out[3]), _stream()), "bts_bn_fold")

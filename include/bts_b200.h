@@ -40,23 +40,14 @@ int bts_version(char *buf, int buflen);
  *     depth[b,y,x] = n4 / ((n1*u(x) + n2*v(y)) + n3),  plane of patch (y/r, x/r),
  *     u(x) = ((x mod r) - (r-1)/2)/r  (bit-exact dyadic grid), v(y) likewise.
  * `focal` is unused by the reference in both implementations (SURVEY Q1) and is not a parameter.
- * Optional fused by-products of bts.forward (pytorch/bts.py:228-229,242-243,256); pass NULL to skip:
- *     scaled = depth / max_depth            (B,H,W)
- *     ds     = scaled[:, ::ds_stride, ::ds_stride]   (B,H/ds_stride,W/ds_stride)  nearest down-sample
- * `depth` itself may be NULL when only the by-products are wanted.  upratio r must be 1 or even. */
+ * upratio r must be 1 or even. */
 int bts_lpg_fwd(const float *plane, float *depth, int B, int h, int w, int r, int layout, void *stream);
-int bts_lpg_fwd_fused(const float *plane, float *depth, float *scaled, float *ds, float max_depth,
-                      int ds_stride, int B, int h, int w, int r, int layout, void *stream);
 
 /* Backward (autograd of pytorch/bts.py:146; custom_layer/local_planar_guidance.cu:95-150, .cc:241-298):
  *     dplane[b,:,i,j] = sum over the r x r tile of (-dY*n4*u/den^2, -dY*n4*v/den^2, -dY*n4/den^2, dY/den)
- * tf_compat=1 drops n4 from the first three (the reference TF kernel's formula, SURVEY Q5).
- * Fused form: dY_total = d_depth + (d_scaled + scatter(d_ds)) / max_depth, any of the three may be NULL. */
+ * tf_compat=1 drops n4 from the first three (the reference TF kernel's formula, SURVEY Q5). */
 int bts_lpg_bwd(const float *dy, const float *plane, float *dplane, int B, int h, int w, int r,
                 int layout, int tf_compat, void *stream);
-int bts_lpg_bwd_fused(const float *d_depth, const float *d_scaled, const float *d_ds, float max_depth,
-                      int ds_stride, const float *plane, float *dplane, int B, int h, int w, int r,
-                      int layout, int tf_compat, void *stream);
 
 /* Host-pointer plugin form of the TF op pair (input (B,h,w,4) NHWC, output (B,h*r,w*r)); copies in/out
  * and synchronises.  Mirrors LocalPlanarGuidanceOp::Compute / LocalPlanarGuidanceGradOp::Compute
@@ -93,7 +84,7 @@ int bts_plane_head_bwd(const float *d_scaled, const float *d_ds, const float *c3
  * only the hi half of the weight / dY operand.  The packed weights are the same for both values.
  *   out[p,co] = act( sum_{tap,ci} pre(x[p (+) tap, ci]) * w[co,ci,tap] )
  *   pre : x*pre_scale[ci]+pre_shift[ci] (folded BatchNorm; both NULL to skip), then ReLU if pre_relu;
- *         zero padding is applied after pre.  upsample2=1 folds a nearest x2 up-sample of the source in.
+ *         zero padding is applied after pre.
  *   act : 0 none, 1 ELU, 2 sigmoid.
  * x: source (B,Hs,Ws,*) with x_pixel_stride floats between pixels (a channel slice of a wider slab is fine);
  * out likewise with out_pixel_stride.  Weights must first be packed (split hi/lo, K-major, 128B-swizzled tiles):
@@ -106,47 +97,41 @@ int bts_conv_n_tile(int Cout);
 long long bts_conv_packed_floats(int n_rows, int k_channels, int KH, int KW);
 int bts_conv_pack_weights(const float *w, long long s_co, long long s_ci, long long s_kh, long long s_kw,
                           int Cout, int Cin, int KH, int KW, int transpose_flip, float *wpack, void *stream);
-int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
-                 int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                 const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
-                 long long out_pixel_stride, int act, int precision, void *stream);
-
-/* bts_conv_fwd that also returns the BatchNorm batch statistics of its output: stat_sum[co] += sum_p out[p,co],
- * stat_sumsq[co] += sum_p out[p,co]^2 (fp64, accumulated with atomics -> zero them first; any Cout, act must be 0).  Replaces a separate
- * bts_bn_stats pass over the tensor just written (torchvision _DenseLayer: conv1 -> norm2, conv2 -> every later norm1). */
-int bts_conv_fwd_stats(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int upsample2, int Cin,
-                       int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                       const float *pre_scale, const float *pre_shift, int pre_relu, float *out,
-                       long long out_pixel_stride, int act, int precision, double *stat_sum, double *stat_sumsq,
-                       void *stream);
-
-/* General form of bts_conv_fwd (replaces cuDNN's strided-dgrad and grouped-convolution paths behind the ResNet / ResNeXt
- * encoders, reference pytorch/bts.py:282-296 via torchvision.models.resnet):
- *   source_mode 0 plain | 1 nearest x2 up-sample folded in | 2 ZERO-STUFFED x2 source with an explicit out_h x out_w output:
- *       with the transposed, tap-flipped packed operator, stride = 1 and pad' = dil*(K-1) - pad this is the input gradient
- *       of a STRIDE-2 convolution whose input was out_h x out_w (x = dY of that layer);
+/* bts_conv_fwd: the forward / dgrad launch above, with
+ *   source_mode 0 plain | 1 nearest x2 up-sample of the source folded in | 2 ZERO-STUFFED x2 source with an explicit
+ *       out_h x out_w output (out_h / out_w are ignored otherwise): with the transposed, tap-flipped packed operator,
+ *       stride = 1 and pad' = dil*(K-1) - pad this is the input gradient of a STRIDE-2 convolution whose input was
+ *       out_h x out_w (x = dY of that layer; replaces cuDNN's strided dgrad behind the ResNet / ResNeXt encoders, reference
+ *       pytorch/bts.py:282-296 via torchvision.models.resnet);
  *   kwin > 0 block-diagonal ("grouped") operator packed by bts_conv_pack_weights_grouped: output channels
- *       [nt*kwin, (nt+1)*kwin) read input channels [nt*kwin, (nt+1)*kwin) only; Cin == Cout == the layer width;
- *   stat_sum / stat_sumsq as in bts_conv_fwd_stats (or both NULL). */
-int bts_conv_fwd_ex(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
-                    int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                    const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
-                    int act, int precision, double *stat_sum, double *stat_sumsq, void *stream);
-/* Split-K form of bts_conv_fwd_ex, for launches whose tiles (128-pixel x n-tile output blocks) leave SMs idle (batch-1
- * inference): each tile's K range is cut into `splits` ranges run by separate CTAs, which write raw fp32 partial tile sums
- * into `workspace` ([splits][M][Cout rounded up to 4], 16-byte aligned); a second kernel adds them in a fixed order (the
- * result is reproducible run to run) and applies `act` into out.  stat_sum / stat_sumsq must be NULL (BTS_EINVAL
- * otherwise): the split kernel has no statistics or BatchNorm-backward epilogue.
+ *       [nt*kwin, (nt+1)*kwin) read input channels [nt*kwin, (nt+1)*kwin) only; Cin == Cout == the layer width; 0 = dense;
+ *   stat_sum / stat_sumsq (both or neither): the BatchNorm batch statistics of the output, stat_sum[co] += sum_p out[p,co],
+ *       stat_sumsq[co] += sum_p out[p,co]^2 (fp64, accumulated with atomics -> zero them first; any Cout, act must be 0).
+ *       Replaces a separate bts_bn_stats pass over the tensor just written (torchvision _DenseLayer: conv1 -> norm2,
+ *       conv2 -> every later norm1);
+ *   x_bn / bn_st (both or neither; needs the statistics pointers and act 0): BatchNorm(+ReLU)-backward epilogue of the
+ *       layer in front of a dgrad.  The tile written is g = dL/d[relu](bn(x_bn)); the statistics pointers receive
+ *       S1[c] += sum_p g*mask and S2[c] += sum_p g*mask*xhat instead (zero them first), mask = [bn(x_bn)>0] when relu
+ *       else 1, xhat = (x_bn-mean)*invstd.  x_bn: the BatchNorm INPUT at the output's pixels and channels, pixel stride
+ *       x_bn_stride; bn_st = [4][Cout] scale|shift|mean|invstd (the bts_bn_finalize layout).  Replaces the
+ *       bts_bn_bwd_reduce pass over (x, g); follow with bts_bn_bwd_coef + bts_bn_bwd_apply;
+ *   workspace != NULL: split-K, for launches whose tiles (128-pixel x n-tile output blocks) leave SMs idle (batch-1
+ *       inference): each tile's K range is cut into `splits` ranges run by separate CTAs, which write raw fp32 partial
+ *       tile sums into `workspace` ([splits][M][Cout rounded up to 4], 16-byte aligned); a second kernel adds them in a
+ *       fixed order (the result is reproducible run to run) and applies `act` into out.  The split kernel has no
+ *       statistics or BatchNorm-backward epilogue: both are refused with a workspace.  workspace == NULL does not split;
+ *       splits must then be 1.
+ * Refused argument combinations return BTS_EINVAL (a misaligned workspace BTS_EALIGN) before any CUDA runtime call.
  *   bts_conv_fwd_splitk_plan(B, Hout, Wout, kwin, Cin, KH, KW, Cout, &splits, &workspace_floats): with *splits = 0 on
  *   entry, the engine's choice (1 = do not split: the launch already fills more than half the SMs, or K is too short);
  *   with *splits = n > 0, n reduced so that no split is empty.  *workspace_floats: the workspace that count needs. */
+int bts_conv_fwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
+                 int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
+                 const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
+                 int act, int precision, double *stat_sum, double *stat_sumsq, const float *x_bn, long long x_bn_stride,
+                 const float *bn_st, int relu, int splits, float *workspace, void *stream);
 int bts_conv_fwd_splitk_plan(int B, int Hout, int Wout, int kwin, int Cin, int KH, int KW, int Cout, int *splits,
                              long long *workspace_floats);
-int bts_conv_fwd_splitk(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
-                        int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                        const float *pre_scale, const float *pre_shift, int pre_relu, float *out, long long out_pixel_stride,
-                        int act, int precision, double *stat_sum, double *stat_sumsq, int splits, float *workspace,
-                        void *stream);
 /* Tuning / bring-up switches of the narrow-output wgrad (csrc/wgrad2_tc.cu).  set_tma(0): the producers load the operands
  * from global memory (round-1 path) instead of the TMA landing ring; set_min_pixels(n): smallest map (input pixels) routed to
  * this kernel (default 12000, n < 0 restores it; tests pass 0 to reach it with small shapes). */
@@ -155,14 +140,7 @@ int bts_wgrad2_set_min_pixels(long long n);
 int bts_wgrad2_set_min_kblocks(int n);
 int bts_wgrad2_set_pointwise(int on);        /* 1 (default): 1x1 layers with 64 < Cout <= 256 use this kernel too */
 
-/* dgrad (or any act-free conv) whose epilogue also reduces the BatchNorm(+ReLU)-backward sums of the layer in front of the
- * conv: the tile written is g = dL/d[relu](bn(x_bn)); S1[c] += sum_p g*mask, S2[c] += sum_p g*mask*xhat (zero them first),
- * mask = [bn(x)>0] when relu else 1, xhat = (x-mean)*invstd; bn_st = [4][Cout] scale|shift|mean|invstd.  Replaces the
- * bts_bn_bwd_reduce pass over (x, g); follow with bts_bn_bwd_coef + bts_bn_bwd_apply. */
-int bts_conv_fwd_bnbwd(const float *x, long long x_pixel_stride, int B, int Hs, int Ws, int source_mode, int out_h, int out_w,
-                       int kwin, int Cin, int KH, int KW, int stride, int pad, int dil, const float *wpack, int Cout,
-                       float *out, long long out_pixel_stride, int precision, const float *x_bn, long long x_bn_stride,
-                       const float *bn_st, int relu, double *S1, double *S2, void *stream);
+/* (k0, k1) of bts_bn_bwd_apply from sums reduced elsewhere (the BatchNorm-backward epilogue of bts_conv_fwd) */
 int bts_bn_bwd_coef(const double *S1, const double *S2, long long M, int C, const float *scale, const float *mean,
                     const float *invstd, float *coef, void *stream);
 /* grouped 3x3 (ResNeXt: 32 groups of cpg channels): w is (width, cpg, KH, KW).  bts_conv_group_window -> the diagonal block
@@ -213,31 +191,21 @@ int bts_conv_c1_wgrad(const float *x, long long x_pixel_stride, const float *dy,
  * backward pass over NHWC tensors (explicit pixel strides -> channel slices of slabs work in place).
  *   bts_bn_stats            : sum / sum of squares per channel (fp64 accumulators, zeroed by the call)
  *   bts_bn_finalize         : -> scale = gamma*invstd, shift = beta - mean*scale, mean, invstd (+ running-stat update,
- *                             momentum m, unbiased variance; running_* may be NULL)
+ *                             momentum m, unbiased variance; running_* may be NULL; num_batches_tracked += 1 unless NULL)
  *   bts_bn_fold             : the same four vectors from frozen running statistics (eval mode)
- *   bts_bn_relu_bwd_reduce  : S1 = sum g*[y>0], S2 = sum g*[y>0]*xhat (y = x*scale+shift) and the fp32 backward
- *                             coefficients coef[0:C] = k0, coef[C:2C] = k1 (dx = [y>0]*scale*g + k1*x + k0)
- *   bts_bn_relu_bwd_apply   : out (=|+=) [y>0]*scale*g + k1*x + k0   (coef == NULL: frozen statistics, k0 = k1 = 0) */
+ *   bts_bn_bwd_reduce       : S1 = sum g*mask, S2 = sum g*mask*xhat (y = x*scale+shift, mask = the backward mask of `act`
+ *                             at y) and the fp32 backward coefficients coef[0:C] = k0, coef[C:2C] = k1
+ *                             (dx = mask*scale*g + k1*x + k0)
+ *   bts_bn_bwd_apply        : out (=|+=) mask*scale*g + k1*x + k0   (coef == NULL: frozen statistics, k0 = k1 = 0)
+ * `act` is the activation after the normalisation: 0 none (plain BatchNorm, as the decoder's bn5/bn4/bn4_2/bn3/bn2 which
+ * feed a concat, bts.py:200-246), 1 ReLU (mask [y>0]), 2 ReLU6 (torchvision mobilenet_v2's Conv2dNormActivation /
+ * InvertedResidual, bts.py:297-300; its backward mask is 0 < y < 6, strictly, as hardtanh_backward). */
 int bts_bn_stats(const float *x, long long x_pixel_stride, long long M, int C, double *sum, double *sumsq, void *stream);
 int bts_bn_finalize(const double *sum, const double *sumsq, long long N, int C, const float *gamma, const float *beta,
-                    float eps, float momentum, float *running_mean, float *running_var, float *scale, float *shift,
-                    float *mean, float *invstd, void *stream);
-int bts_bn_finalize_track(const double *sum, const double *sumsq, long long N, int C, const float *gamma, const float *beta,
-                          float eps, float momentum, float *running_mean, float *running_var, long long *num_batches_tracked,
-                          float *scale, float *shift, float *mean, float *invstd, void *stream);   /* + num_batches_tracked += 1 */
+                    float eps, float momentum, float *running_mean, float *running_var, long long *num_batches_tracked,
+                    float *scale, float *shift, float *mean, float *invstd, void *stream);
 int bts_bn_fold(int C, const float *gamma, const float *beta, float eps, const float *running_mean,
                 const float *running_var, float *scale, float *shift, float *mean, float *invstd, void *stream);
-int bts_bn_relu_bwd_reduce(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
-                           long long M, int C, const float *scale, const float *shift, const float *mean,
-                           const float *invstd, double *S1, double *S2, float *coef, void *stream);
-int bts_bn_relu_bwd_apply(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride,
-                          long long M, int C, const float *scale, const float *shift, const float *coef, float *out,
-                          long long out_pixel_stride, int accumulate, void *stream);
-
-/* generalised forms with an explicit activation code `act`: 0 none (plain BatchNorm, as the decoder's bn5/bn4/bn4_2/bn3/bn2
- * which feed a concat, bts.py:200-246), 1 ReLU, 2 ReLU6 (torchvision mobilenet_v2's Conv2dNormActivation / InvertedResidual,
- * bts.py:297-300; its backward mask is 0 < y < 6, strictly, as hardtanh_backward); the *_relu_* entry points above are these
- * with act=1. */
 int bts_bn_bwd_reduce(const float *x, long long x_pixel_stride, const float *g, long long g_pixel_stride, long long M,
                       int C, const float *scale, const float *shift, const float *mean, const float *invstd, int act,
                       double *S1, double *S2, float *coef, void *stream);

@@ -265,7 +265,8 @@ def test_pointwise_wgrad_cuda_core_kernel(Cin, Cout, monkeypatch):
 @pytest.mark.parametrize("Cin,Cout,k,H,W,act", [(40, 48, 3, 13, 21, None), (96, 192, 1, 9, 14, None), (36, 32, 3, 20, 28, None),
                                                  (64, 256, 1, 8, 8, None)])
 def test_conv_epilogue_batch_statistics(Cin, Cout, k, H, W, act):
-    """per-channel sum / sum of squares of the conv output reduced in the epilogue (bts_conv_fwd_stats) == a separate pass"""
+    """per-channel sum / sum of squares of the conv output reduced in the epilogue (bts_conv_fwd with stat_sum /
+    stat_sumsq) == a separate pass"""
     from bts_b200 import conv
     g = torch.Generator().manual_seed(21)
     x = torch.randn(3, Cin, H, W, generator=g).cuda().contiguous(memory_format=torch.channels_last)

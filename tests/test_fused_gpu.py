@@ -27,7 +27,7 @@ def _block(C0, L, growth=48, bn_size=4):
 def epi_bnbwd(request):
     """the three forms of the dense-layer BatchNorm backward: one streaming pass with the per-channel affine remainder
     deferred (default, bts_bn_relu_bwd_fused + bts_bn_bwd_correct), reduce pass + apply pass, and the sums reduced in the
-    dgrad epilogue (bts_conv_fwd_bnbwd)"""
+    dgrad epilogue (bts_conv_fwd with x_bn / bn_st)"""
     from bts_b200 import fused
     prev = fused.EPI_BNBWD, fused.BN_ONEPASS
     fused.EPI_BNBWD = request.param == "epilogue"

@@ -97,3 +97,29 @@ def test_packed_operator_sizes_and_group_windows():
         assert L.bts_conv_group_window(width, cpg) == 128
     assert L.bts_conv_group_window(96, 3) == 96                   # narrower widths: one window
     assert L.bts_conv_group_window(100, 3) == 0                   # width not a multiple of the group size: refused
+
+
+def test_conv_fwd_refuses_conflicting_epilogues_before_any_launch():
+    """bts_conv_fwd refuses every argument combination its epilogues cannot serve; with fake, 16-byte aligned device
+    addresses each call must return before it touches the device"""
+    L = _lib()
+    EINVAL, EALIGN = -1, -2
+    p = ctypes.c_void_p(1 << 20)
+
+    def fwd(stats=(None, None), act=0, bn=(None, None), splits=1, ws=None):
+        # a 3x3 32 -> 32 layer on one 8 x 8 image: every geometry argument is valid
+        return L.bts_conv_fwd(p, 32, 1, 8, 8, 0, 0, 0, 0, 32, 3, 3, 1, 1, 1, p, 32, None, None, 0, p, 32, act, 0,
+                              stats[0], stats[1], bn[0], 32, bn[1], 1, splits, ws, None)
+
+    assert fwd(stats=(p, p), splits=2, ws=p) == EINVAL             # split-K with statistics
+    assert fwd(stats=(p, p), bn=(p, p), splits=2, ws=p) == EINVAL  # split-K with the BatchNorm-backward epilogue
+    assert fwd(bn=(p, p)) == EINVAL                                # BatchNorm-backward without its sums
+    assert fwd(stats=(p, p), bn=(p, p), act=1) == EINVAL           # BatchNorm-backward after an activation
+    assert fwd(stats=(p, p), bn=(p, None)) == EINVAL               # half the BatchNorm-backward operands
+    assert fwd(stats=(p, p), bn=(None, p)) == EINVAL
+    assert fwd(stats=(p, p), act=2) == EINVAL                      # statistics of an activated output
+    assert fwd(stats=(p, None)) == EINVAL                          # one of the two statistics pointers
+    assert fwd(stats=(None, p)) == EINVAL
+    assert fwd(splits=2) == EINVAL                                 # splits without a workspace
+    assert fwd(splits=0) == EINVAL
+    assert fwd(splits=2, ws=ctypes.c_void_p((1 << 20) + 4)) == EALIGN   # misaligned workspace
