@@ -132,6 +132,8 @@ SIGNATURES = {
     "bts_dw3x3_dgrad": [_p, _ll, _i, _i, _i, _i, _i, _p, _ll, _ll, _ll, _p, _ll, _p],
     "bts_dw3x3_wgrad_workspace_floats": [_i, _i, _i, _i, _i],
     "bts_dw3x3_wgrad": [_p, _ll, _p, _ll, _i, _i, _i, _i, _i, _p, _p, _p, _p, _ll, _ll, _ll, _p],
+    "bts_png_inflate": [_p, _p, _i, _i, _p, _p, _p, _p],
+    "bts_png_unfilter": [_p, _p, _p, _i, _i, _i, _i, _p, _p, _p],
 }
 RESTYPES = {"bts_conv_packed_floats": ctypes.c_longlong, "bts_conv_packed_floats_grouped": ctypes.c_longlong, "bts_conv_pw_wgrad_workspace_floats": ctypes.c_longlong,
             "bts_dw3x3_fwd_workspace_floats": ctypes.c_longlong, "bts_dw3x3_wgrad_workspace_floats": ctypes.c_longlong}

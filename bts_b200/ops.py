@@ -6,6 +6,7 @@ or CPU fallback -- non-CUDA inputs raise.
 """
 import ctypes
 
+import numpy as np
 import torch
 
 from . import _lib, data
@@ -224,4 +225,78 @@ def depth_to_u16(depth, scale):
     out = torch.empty(depth.shape, device=depth.device, dtype=torch.uint16)
     _lib.check(_lib.lib().bts_depth_to_u16(_ptr(depth), float(scale), depth.numel(), _ptr(out), _stream()), "bts_depth_to_u16")
     _lib.count()
+    return out
+
+
+_PNG_REASONS = {1: "truncated stream", 2: "bad zlib header", 3: "bad DEFLATE block", 4: "bad Huffman code table",
+                5: "distance too far back", 6: "wrong decompressed size", 7: "Adler-32 mismatch", 8: "bad filter type"}
+
+
+def decode_png(blobs, origins=None, out_hw=None):
+    """Decodes a batch of PNG files on the current CUDA device and stream, cropped: what
+    np.stack([np.asarray(Image.open(f))[y0:y0 + Hc, x0:x0 + Wc] ...]) gives, as (B, Hc, Wc, 3) uint8 for 8-bit RGB or
+    (B, Hc, Wc) uint16 in native byte order for 16-bit grayscale (the inputs of input_prep).
+
+    blobs: the files' bytes, all of one format.  origins: None or one (y0, x0) per file; out_hw: None or (Hc, Wc).
+    Without out_hw every frame must have the same size and the window is the frame less its origin; with the training
+    recipe the windows are data.fixed_crop_box(dataset, do_kb_crop, h, w).
+
+    The container is checked on the host (data.parse_png) before anything reaches the device.  The streams go to the device
+    in one pinned host-to-device copy, with one copy of the per-image metadata; bts_png_inflate and bts_png_unfilter run on
+    the current stream.  The call then synchronises once, to read each image's status back: a stream that fails to decode
+    raises ValueError naming the first failing image's index and reason, and leaves nothing behind."""
+    blobs = list(blobs)
+    if not blobs:
+        raise ValueError("decode_png needs at least one PNG")
+    parsed = [data.parse_png(b) for b in blobs]
+    fmt, bpp = parsed[0][0], parsed[0][1]
+    for i, p in enumerate(parsed):
+        if p[0] != fmt:
+            raise ValueError("decode_png takes one format per call: image 0 is %s, image %d is %s" % (fmt, i, p[0]))
+    n = len(parsed)
+    if origins is None:
+        origins = [(0, 0)] * n
+    origins = [(int(y), int(x)) for y, x in origins]
+    if len(origins) != n:
+        raise ValueError("origins must hold one (y0, x0) per image (%d), got %d" % (n, len(origins)))
+    if out_hw is None:
+        sizes = {p[2:4] for p in parsed}
+        if len(sizes) != 1:
+            raise ValueError("without out_hw every frame must have the same size, got %s" % sorted(sizes))
+        h, w = sizes.pop()
+        if len(set(origins)) != 1:
+            raise ValueError("without out_hw every image must have the same origin")
+        out_hw = (h - origins[0][0], w - origins[0][1])
+    Hc, Wc = int(out_hw[0]), int(out_hw[1])
+    meta = np.zeros((n, 8), dtype=np.int64)
+    src_off = raw_off = 0
+    for i, ((_, _, h, w, stream), (y0, x0)) in enumerate(zip(parsed, origins)):
+        if Hc < 1 or Wc < 1 or y0 < 0 or x0 < 0 or y0 + Hc > h or x0 + Wc > w:
+            raise ValueError("image %d: the crop (%d, %d, %d, %d) is outside its %dx%d frame" % (i, y0, x0, Hc, Wc, h, w))
+        meta[i] = (src_off, len(stream), raw_off, h, w, y0, x0, 0)
+        src_off += len(stream)
+        raw_off += h * (1 + w * bpp)
+    dev = torch.device("cuda", torch.cuda.current_device())
+    host = torch.empty(max(src_off, 1), dtype=torch.uint8, pin_memory=True)
+    hv = host.numpy()
+    for i, p in enumerate(parsed):
+        hv[meta[i, 0]:meta[i, 0] + meta[i, 1]] = np.frombuffer(p[4], dtype=np.uint8)
+    src = host.to(dev, non_blocking=True)
+    meta_d = torch.from_numpy(meta).to(dev)
+    raw = torch.empty(raw_off, dtype=torch.uint8, device=dev)
+    work = torch.empty(2 * n, dtype=torch.int32, device=dev)   # status [n], stored Adler-32 [n]
+    out = torch.empty((n, Hc, Wc, 3) if bpp == 3 else (n, Hc, Wc), dtype=torch.uint8 if bpp == 3 else torch.uint16,
+                      device=dev)
+    L = _lib.lib()
+    status, adler = work[:n], work[n:]
+    _lib.check(L.bts_png_inflate(_ptr(src), _ptr(meta_d), n, bpp, _ptr(raw), _ptr(adler), _ptr(status), _stream()),
+               "bts_png_inflate")
+    _lib.check(L.bts_png_unfilter(_ptr(raw), _ptr(meta_d), _ptr(adler), n, bpp, Hc, Wc, _ptr(out), _ptr(status),
+                                  _stream()), "bts_png_unfilter")
+    _lib.count(2)
+    st = status.cpu().numpy()   # the one synchronisation of the call
+    bad = np.nonzero(st)[0]
+    if len(bad):
+        i = int(bad[0])
+        raise ValueError("decode_png: image %d: %s (status %d)" % (i, _PNG_REASONS.get(int(st[i]), "unknown"), int(st[i])))
     return out

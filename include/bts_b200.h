@@ -350,6 +350,36 @@ int bts_eval_errors(const float *pred, const float *gt, int H, int W, float min_
                     int crop_y1, int crop_x0, int crop_x1, double *workspace, float *metrics_out, void *stream);
 int bts_depth_to_u16(const float *depth, float scale, long long n, unsigned short *out, void *stream);
 
+/* ---- batched PNG decode, csrc/png.cu (decode core: csrc/png_core.cuh)
+ * The training PNGs (KITTI RGB, KITTI / NYU 16-bit depth) decoded on the device, cropped to a per-image window.  The host
+ * (bts_b200.data.parse_png) checks the container and concatenates each file's IDAT payloads into one zlib stream.
+ *   src:   device bytes, the n zlib streams packed back to back.
+ *   meta:  device long long [n][8] = src offset, src length, raw offset, height, width, crop y0, crop x0, 0.
+ *   bpp:   3 (RGB, 8 bit) or 2 (grayscale, 16 bit).
+ *   raw:   device bytes, per image the filtered scanlines, height * (1 + width * bpp) bytes at its raw offset.
+ *   adler: device unsigned [n], the Adler-32 each stream stores (written by bts_png_inflate).
+ *   out:   device (n, out_h, out_w, 3) uint8 or (n, out_h, out_w) uint16 in native byte order; image i is its frame's
+ *          window rows [y0, y0 + out_h), columns [x0, x0 + out_w).
+ *   status: device int [n]; bts_png_inflate writes one BTS_PNG_* per image, bts_png_unfilter decodes the images whose
+ *          status is BTS_PNG_OK and may set BTS_PNG_ADLER_MISMATCH or BTS_PNG_BAD_FILTER.  Malformed data only ever sets
+ *          a status: the kernels neither trap nor touch memory outside these buffers.
+ * Limits: width * bpp <= BTS_PNG_MAX_ROW_BYTES (bts_png_unfilter keeps two rows in shared memory); each image's raw
+ * size <= 2^28 bytes.  Bad arguments (n <= 0, a null pointer, another bpp, out_h or out_w <= 0) return BTS_EINVAL. */
+#define BTS_PNG_MAX_ROW_BYTES 16384
+#define BTS_PNG_OK 0
+#define BTS_PNG_TRUNCATED 1         /* the stream ends before its end-of-stream marker or Adler-32 */
+#define BTS_PNG_BAD_ZLIB_HEADER 2   /* CM != 8, CINFO > 7, FCHECK fails or a preset dictionary */
+#define BTS_PNG_BAD_BLOCK 3         /* block type 3, or a stored block whose LEN and NLEN disagree */
+#define BTS_PNG_BAD_CODE_TABLE 4    /* invalid Huffman code lengths, or a code the block's tables do not define */
+#define BTS_PNG_DISTANCE_TOO_FAR 5  /* a match reaches before the start of the output */
+#define BTS_PNG_BAD_SIZE 6          /* decompressed size differs from height * (1 + width * bpp) */
+#define BTS_PNG_ADLER_MISMATCH 7    /* Adler-32 of the decompressed bytes differs from the stored one */
+#define BTS_PNG_BAD_FILTER 8        /* a row's filter type byte is > 4 */
+int bts_png_inflate(const unsigned char *src, const long long *meta, int n, int bpp, unsigned char *raw, unsigned int *adler,
+                    int *status, void *stream);
+int bts_png_unfilter(const unsigned char *raw, const long long *meta, const unsigned int *adler, int n, int bpp, int out_h,
+                     int out_w, void *out, int *status, void *stream);
+
 /* zero n floats on the stream (grad_focal output of the TF-op surface, integration/tf_op/bts_lpg_tf_op.cc) */
 int bts_fill_zero_f32(float *p, long long n, void *stream);
 
